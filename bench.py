@@ -4,12 +4,17 @@
     python bench.py --gpus N --steps K --warmup W            # this implementation
     python bench.py --impl reference --steps K --warmup W    # CPU restatement of the reference step
 
-N=1 workload: BASELINE.json configs[1] (ResNet-50 1x, batch 512 per GPU,
-224x224 synthetic, proj_dim 128, temperature 0.1, LARS, blur + linear-eval head
-on, SyncBN flag on).  Under torchrun (N>1) every rank keeps 512 samples (weak
-scaling; N=8 is configs[2], global batch 4096).  A "step" is one complete
+N=1 workload: ResNet-50 1x, batch 256 per GPU (what one 80 GB H100 holds next
+to the profiling pass), 224x224 synthetic, proj_dim 128, temperature 0.1, LARS,
+blur + linear-eval head on, SyncBN flag on.  Under torchrun (N>1) every rank
+keeps 256 samples (weak scaling).  A "step" is one complete
 `single_step` (tf2/run.py:557-622): forward, NT-Xent, backward, gradient
 all-reduce, LARS.  One JSON line is printed by rank 0.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step
+computed: its loss and a fixed, seeded sample of every updated trainable
+variable, as DIR/<name>.npy (float64 / float32), so that two builds can be
+compared output for output on identical seeded inputs.
 """
 import argparse
 import json
@@ -34,13 +39,13 @@ def parse_args():
     ap.add_argument('--steps', type=int, default=10)
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--impl', default='b200', choices=['b200', 'reference'])
-    ap.add_argument('--batch', type=int, default=512, help='samples per GPU')
+    ap.add_argument('--batch', type=int, default=256, help='samples per GPU')
     ap.add_argument('--resnet_depth', type=int, default=50)
     ap.add_argument('--width_multiplier', type=int, default=1)
     ap.add_argument('--image_size', type=int, default=224)
     ap.add_argument('--precision', default='bf16', choices=['bf16', 'fp32'])
     ap.add_argument('--engine', default='tc', choices=['tc', 'tc3', 'simt'],
-                    help='tc: bf16 tcgen05 (the benchmarked mode); tc3: fp32-accurate split-bf16 tcgen05 (needs --precision fp32)')
+                    help='tc: bf16 wgmma (the benchmarked mode); tc3: fp32-accurate split-bf16 wgmma (needs --precision fp32)')
     ap.add_argument('--sk_ratio', type=float, default=0.0, help='config 5: 0.0625')
     ap.add_argument('--num_proj_layers', type=int, default=3)
     ap.add_argument('--learning_rate', type=float, default=0.3)
@@ -50,6 +55,8 @@ def parse_args():
     ap.add_argument('--no_cpu_baseline', action='store_true')
     ap.add_argument('--cpu_batch', type=int, default=16)
     ap.add_argument('--cpu_steps', type=int, default=2)
+    ap.add_argument('--dump-outputs', dest='dump_outputs', default=None, metavar='DIR',
+                    help='write the last timed step\'s outputs as DIR/<name>.npy')
     return ap.parse_args()
 
 
@@ -65,7 +72,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(tflops=d['bf16_tflops_sustained'], hbm=d['hbm_gbs'], which='measured (sustained bf16, MEASURED_PEAKS.json)')
-    return dict(tflops=1400.0, hbm=6650.0, which='fallback (B200_PROFILING.md)')
+    return dict(tflops=989.0, hbm=3350.0, which='H100 SXM data sheet (dense bf16, HBM3; 700 W), not a measured peak')
 
 
 class ClockSampler(threading.Thread):
@@ -177,6 +184,9 @@ def run_b200(args):
 
     rank = run.init_distributed()
     log('process group ready')
+    # the per-step random draws of the step (blur sigma / selector) come from torch's default generators: seed them,
+    # so that the same arguments give the same inputs, and the same outputs, on every run
+    torch.manual_seed(1234 + rank)
     world = dist.get_world_size() if dist.is_initialized() else 1
     local = int(os.environ.get('LOCAL_RANK', '0'))
     torch.cuda.set_device(local)
@@ -280,6 +290,9 @@ def run_b200(args):
     loss_val = float(loss)
 
     log('timed region done: %.2f ms/step' % ms_per_step + ('' if sync_wait is None else ' peer-wait ms/step per rank %s' % sync_wait))
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, loss, trainer.model.trainable_variables)
+        log('outputs written to %s' % args.dump_outputs)
     # ---- e2e: host buffers, H2D inside the timed region, D2H of the loss ------
     host_f = [torch.rand(B, S, S, 6).pin_memory() for _ in range(2)]
     host_l = [labels.cpu().pin_memory() for _ in range(2)]
@@ -328,7 +341,7 @@ def run_b200(args):
     h2d_bytes = features.numel() * 4 + labels.numel() * 4
 
     log('e2e done')
-    # ---- roofline pass: per-launch CUDA-event timing of the tcgen05 kernels ----
+    # ---- roofline pass: per-launch CUDA-event timing of the tensor-core kernels ----
     roof = None
     # every rank runs the profiled step (it contains collectives); rank 0 reports its own timings
     eng.profile = []
@@ -342,31 +355,18 @@ def run_b200(args):
             d[0] += flops; d[1] += a.elapsed_time(b) * 1e-3; d[2] += 1
         tot_f = sum(v[0] for v in by.values()); tot_t = sum(v[1] for v in by.values())
         achieved = tot_f / tot_t / 1e12 if tot_t > 0 else 0.0
-        # algorithmic bytes of the conv kernels (activations in + out once, packed weights once) and, when the
-        # committed ncu capture matches this workload, the DRAM traffic it measured (profiles/traffic.json)
+        # algorithmic bytes of the conv kernels (activations in + out once, packed weights once)
         alg = 0.0
         for kind, shape, flops, a, b in eng.profile:
             n_, h_, w_, ci, co, r_, s_ = shape
             ho, wo = (h_ - 1) // s_ + 1, (w_ - 1) // s_ + 1
             alg += 2.0 * (n_ * h_ * w_ * ci + n_ * ho * wo * co + r_ * r_ * ci * co)
         n_launch = max(len(eng.profile), 1)
-        traffic = None; traffic_src = None
-        tj = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'profiles', 'traffic.json')
-        if os.path.exists(tj) and args.resnet_depth == 50 and args.width_multiplier == 1 and B == 512 and S == 224 \
-                and args.sk_ratio == 0 and args.engine == 'tc':
-            try:
-                tr = json.load(open(tj))
-                # per conv CALL of this run (a strided dgrad call is up to 4 parity-class kernels: ncu counts
-                # tr['launches'] kernels for the n_launch calls timed here)
-                traffic = tr['dram_bytes_per_step'] / n_launch
-                traffic_src = 'profiles/traffic.json (%s; %d kernel launches for %d conv calls)' % (tr['source'], tr['launches'], n_launch)
-            except Exception:
-                traffic = None
         key = (args.resnet_depth, args.width_multiplier, S, args.sk_ratio > 0)
         step_tflops = (ips / world) * GFLOP_PER_IMAGE[key] / 1e3 if key in GFLOP_PER_IMAGE else None
-        roof = {'bound': 'tensor', 'kernel': 'igemm / wgrad / halo3x3 / stem7x7 kernels (tcgen05 implicit GEMM, %d conv calls per step)' % sum(v[2] for v in by.values()),
+        roof = {'bound': 'tensor', 'kernel': 'igemm / wgrad / halo3x3 / stem7x7 kernels (wgmma implicit GEMM, %d conv calls per step)' % sum(v[2] for v in by.values()),
                 'achieved': achieved, 'peak': peaks['tflops'], 'unit': 'TFLOP/s', 'frac': achieved / peaks['tflops'],
-                'traffic': traffic, 'traffic_source': traffic_src, 'algorithmic_bytes': alg / n_launch,
+                'algorithmic_bytes': alg / n_launch,
                 'peak_source': peaks['which'],
                 'conv_share_of_step': tot_t * 1e3 / ms_per_step,
                 'conv_kernel_ms': tot_t * 1e3,
@@ -399,7 +399,7 @@ def run_b200(args):
                     l2v = tr2.single_step(f2, l2)
                 b.record(); torch.cuda.synchronize()
                 ms2 = a.elapsed_time(b) / n2
-                secondary = {'engine': 'tc3 (three-way split-bf16 products on tcgen05, fp32 storage; 1e-3 step parity: '
+                secondary = {'engine': 'tc3 (three-way split-bf16 products on wgmma, fp32 storage; 1e-3 step parity: '
                                        'tests/test_gpu_step.py::test_step_parity_tc3)',
                              'value': b2 / (ms2 / 1e3), 'unit': 'images/s', 'batch': b2, 'ms_per_step': ms2, 'steps': n2,
                              'cuda_graph': False, 'loss': float(l2v)}
@@ -442,6 +442,24 @@ def run_b200(args):
         emit(line)
     if dist.is_initialized():
         dist.destroy_process_group()
+
+
+DUMP_SAMPLE = 4096          # elements kept per variable (a fixed, seeded sample of the larger ones)
+
+
+def dump_outputs(out_dir, loss, variables):
+    """The loss of the last timed step and the variables it updated, as .npy files (at most a few MB)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, 'loss.npy'), np.array([float(loss)], dtype=np.float64))
+    g = torch.Generator().manual_seed(0)
+    for v in variables:
+        flat = v.value.detach().reshape(-1).float().cpu()
+        if flat.numel() > DUMP_SAMPLE:
+            flat = flat[torch.randperm(flat.numel(), generator=g)[:DUMP_SAMPLE].sort().values]
+        name = v.name.replace('/', '.').replace(':', '_')
+        np.save(os.path.join(out_dir, name + '.npy'), flat.numpy().astype(np.float32))
 
 
 def _watchdog(seconds):

@@ -1,5 +1,5 @@
 /*
- * simclr_b200 -- C-ABI of the B200-native SimCLR pretrain step.
+ * simclr_b200 -- C-ABI of the H100-native SimCLR pretrain step.
  *
  * The reference (google-research/simclr) has no FFI layer: its hot path is
  * Python calling TensorFlow ops.  This header is therefore the *new* boundary
@@ -247,7 +247,7 @@ SIMCLR_API int simclr_global_avgpool_bwd(const void* dy, int dy_dtype, void* dx,
  *   y  [N,Ho,Wo,Cout], Ho = H (stride 1) or (H-1)/stride+1 with pad (k-1)/2
  * ------------------------------------------------------------------------- */
 
-/* tcgen05 engine operands: K-major packed copies of the fp32 HWIO master.
+/* tensor-core engine operands: K-major packed copies of the fp32 HWIO master.
  *   wf [Cout][Kp]       k = (r*S+s)*Cs + c,   Kp = round_up(R*S*Cs, 128B/elt)
  *                       bf16 with Cs == 4 (the stem: 3 image channels + 1 zero):
  *                       k = (r*(S+1) + s+1)*4 + c, Kp = round_up(R*(S+1)*4, 64); slot 0 of each
@@ -281,7 +281,7 @@ SIMCLR_API int simclr_conv2d_wgrad_tc(const void* x, const void* dy, float* dw, 
                                       int64_t S, int64_t stride, void* stream);
 
 /* Split-bf16 products -- the tensor-core VERIFICATION mode (`--b200_conv_engine=tc3`: fp32 storage,
- * 1e-3 step parity with the fp32 reference of tf2/run.py:557-622 on the tcgen05 pipe).  Every fp32
+ * 1e-3 step parity with the fp32 reference of tf2/run.py:557-622 on the tensor-core pipe).  Every fp32
  * operand v is split three ways, v = v0 + v1 + v2 with v0 = bf16(v), v1 = bf16(v - v0),
  * v2 = bf16(v - v0 - v1) (`simclr_split_bf16x3`; `simclr_pack_conv_weight_part` writes part 0 / 1 / 2
  * of the packed weights in the layouts of `simclr_pack_conv_weight`), and a product is taken as
@@ -305,7 +305,7 @@ SIMCLR_API int simclr_conv2d_wgrad_tc3(const void* x0, const void* x1, const voi
                                        int64_t stride, void* stream);
 
 /* CUDA-core fp32 engine reading the fp32 HWIO master directly (verification
- * engine for the tcgen05 path; not the default). */
+ * engine for the tensor-core path; not the default). */
 SIMCLR_API int simclr_conv2d_fprop_simt(const void* x, const float* w_hwio, void* y, int dtype, int y_dtype,
                                         int64_t N, int64_t H, int64_t W, int64_t Cs, int64_t Cin,
                                         int64_t Cout, int64_t R, int64_t S, int64_t stride, void* stream);

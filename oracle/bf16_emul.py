@@ -14,7 +14,7 @@ CUDA path writes a bf16 tensor to HBM, in the forward AND in the backward pass:
   qw(w)  weight operand: forward value rounded (the packed bf16 copy), gradient in fp32
 
 With it the oracle answers two separate questions the fp32 oracle cannot:
-  1. does the bf16 tcgen05 step compute the bf16-storage algorithm correctly?
+  1. does the bf16 tensor-core step compute the bf16-storage algorithm correctly?
      (CUDA bf16 step vs emulating oracle: only accumulation order and rare rounding
      flips differ)
   2. what does bf16 storage itself cost on a given fixture?

@@ -1,7 +1,7 @@
 """Per-kernel device time of ONE eager pretrain step, from CUPTI activity records (torch.profiler).
 
 Unlike the ncu launch list this runs at full clocks with warm caches and back-to-back launches,
-so the absolute times add up to the eager step time.  Output: gpurun_out/kernel_times.txt
+so the absolute times add up to the eager step time.  Output: kernel_times.txt (or --out)
 """
 import argparse, collections, os, re, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -14,7 +14,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument('--batch', type=int, default=512)
 ap.add_argument('--resnet_depth', type=int, default=50)
 ap.add_argument('--image_size', type=int, default=224)
-ap.add_argument('--out', default=os.path.join(ROOT, 'gpurun_out', 'kernel_times.txt'))
+ap.add_argument('--out', default='kernel_times.txt')
 args = ap.parse_args()
 flags_def.FLAGS(['kernel_times'])
 rank = run.init_distributed()                     # under torchrun: the N>1 step (peer-memory SyncBN, overlapped NCCL)

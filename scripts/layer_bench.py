@@ -1,4 +1,4 @@
-"""Per-layer timing of the tcgen05 engine on the ResNet-50 conv shapes (SURVEY 10.1).
+"""Per-layer timing of the wgmma engine on the ResNet-50 conv shapes (SURVEY 10.1).
 Usage: python scripts/layer_bench.py [--views 256] [--only fprop,dgrad,wgrad] [--out file]"""
 import argparse, os, sys, json
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

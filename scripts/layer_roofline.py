@@ -1,7 +1,7 @@
 """Per-layer roofline reading of a scripts/layer_bench.py log: measured time against
 max(tensor time at the measured bf16 peak, HBM time of the minimum traffic).
 
-  python scripts/layer_roofline.py profiles/r01_layers_im2col.txt [MEASURED_PEAKS.json] > profiles/r01_layer_roofline.txt
+  python scripts/layer_roofline.py layers.txt [MEASURED_PEAKS.json] > layer_roofline.txt
 Layer timings are kernels run alone (L2 flushed), so the burst bf16 figure is the tensor denominator."""
 import json, os, re, sys
 
@@ -11,7 +11,7 @@ pk = sys.argv[2] if len(sys.argv) > 2 else os.path.join(ROOT, 'MEASURED_PEAKS.js
 if os.path.exists(pk):
     d = json.load(open(pk)); TF, HBM, src = d['bf16_tflops'], d['hbm_gbs'], 'MEASURED_PEAKS.json (burst bf16 %.1f TFLOP/s, copy %.1f GB/s)' % (d['bf16_tflops'], d['hbm_gbs'])
 else:
-    TF, HBM, src = 1700.0, 6650.0, 'fallback peaks'
+    TF, HBM, src = 989.0, 3350.0, 'H100 SXM data-sheet peaks (dense bf16, HBM3)'
 pat = re.compile(r'^\s*(\d+)\s+(fprop|dgrad|wgrad)\s+H\s*(\d+)\s+(\d+)->\s*(\d+)\s+k(\d)\s+s(\d)\s+x(\d+)\s+M=\s*(\d+)\s+([\d.]+) ms\s+([\d.]+) TF/s\s+([\d.]+) GB/s')
 rows = []
 for line in open(log):

@@ -1,8 +1,8 @@
-"""In-tree nvcc build of libsimclr_b200.so (sm_100a only).
+"""In-tree nvcc build of libsimclr_b200.so (sm_90a only: H100).
 
 `python -m simclr_b200.build` or `__graft_entry__.build()`.  Objects go to
 `simclr_b200/csrc/_build/`, the shared library to `simclr_b200/libsimclr_b200.so`
-(git-ignored, travels to the GPU box with the snapshot).
+(both git-ignored; a checkout builds them once).
 """
 import hashlib
 import os
@@ -16,7 +16,8 @@ OUT = os.path.join(HERE, 'libsimclr_b200.so')
 BUILD = os.path.join(CSRC, '_build')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 
-FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
+FLAGS = ARCH + ['-lineinfo', '-O3', '-std=c++17',
          '-Xcompiler', '-fPIC,-fvisibility=hidden', '--expt-relaxed-constexpr',
          '-Xptxas', '-v' if os.environ.get('SIMCLR_PTXAS_V') else '-O3']
 
@@ -60,8 +61,7 @@ def build(force=False, verbose=False):
 
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         objs = list(ex.map(compile_one, _sources()))
-    cmd = [NVCC, '-shared', '-o', OUT] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a',
-                                                  '-Xcompiler', '-fPIC']
+    cmd = [NVCC, '-shared', '-o', OUT] + objs + ARCH + ['-Xcompiler', '-fPIC']
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout + r.stderr)

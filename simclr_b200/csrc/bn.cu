@@ -1,6 +1,6 @@
 // BatchNorm family (tf2/resnet.py:31-78; SURVEY.md A4).  All HBM-bound:
 // 16-byte vector loads, per-thread fp32 partials, block tree in shared memory,
-// one double atomicAdd per channel per block.  Tensors are [rows][C] views of
+// one fp64 partial per channel per block, added in block order.  Tensors are [rows][C] views of
 // NHWC activations; C % 8 == 0.
 #include "common.cuh"
 
@@ -254,7 +254,7 @@ bn_reduce_kernel(T* __restrict__ a, const void* __restrict__ a2_, const void* __
           acc += 2.0 * pvt * a0 + n * pvt * pvt;
         }
       }
-      atomicAdd(&sums[(e >> 3) * C + ch], acc);
+      sums[(size_t)blockIdx.x * 2 * C + (e >> 3) * C + ch] = acc;       // this block's partial (summed in block order)
     }
     if (MODE == 4) {        // second tree: (sum dz, sum dz*xhat2) of the shortcut's BatchNorm
       __syncthreads();
@@ -267,7 +267,7 @@ bn_reduce_kernel(T* __restrict__ a, const void* __restrict__ a2_, const void* __
         if (c8 >= cvecs) continue;
         double acc = 0.0;
         for (int l = 0; l < row_lanes; ++l) acc += sh[((size_t)l * P + px) * 16 + e];
-        atomicAdd(&sums2[(e >> 3) * C + c8 * 8 + (e & 7)], acc);
+        sums2[(size_t)blockIdx.x * 2 * C + (e >> 3) * C + c8 * 8 + (e & 7)] = acc;
       }
     }
   }
@@ -517,8 +517,8 @@ int launch_reduce(void* a, const void* a2, const void* zmask, const void* y, int
   const RedLayout l = red_layout(C);
   int64_t nblocks = (rows + l.row_lanes * 8 - 1) / (l.row_lanes * 8);
   // 2 CTAs of 256 threads are resident per SM (__launch_bounds__(BT, 2)): one wave of fat blocks.  Every block ends
-  // with one fp64 atomic per column, and same-address atomics serialise in L2 (~30 ns each): 8 waves of blocks
-  // cost ~30 us of atomic tail per launch, one wave a quarter of that.
+  // with one fp64 partial per column; the partials are added in block order (the same bits every run), so fewer
+  // blocks also mean less to add.
   const int64_t cap = (int64_t)num_sms() * 2;
   if (nblocks > cap) nblocks = cap;
   if (nblocks < 1) nblocks = 1;
@@ -533,10 +533,22 @@ int launch_reduce(void* a, const void* a2, const void* zmask, const void* y, int
       if (e != cudaSuccess) { set_error("bn reduce memset: %s", cudaGetErrorString(e)); return (int)e; }
     }
   }
-  bn_reduce_kernel<T, Ty, MODE><<<(unsigned)nblocks, BT, smem, st>>>(
-      (T*)a, a2, zmask, (const Ty*)y, rows, (int)C, l.P, rows_per_block, mean, rstd, sums, (const Ty*)y2, mean2, rstd2, sums2);
-  SIMCLR_CHECK_LAUNCH();
-  return SIMCLR_OK;
+  const int64_t part = 2 * C;                     // doubles per block partial
+  const int nsets = sums2 ? 2 : 1;
+  double* ws = nullptr;
+  { int rc = scratch_alloc(&ws, (size_t)nsets * nblocks * part * sizeof(double), st); if (rc) return rc; }
+  double* ws2 = sums2 ? ws + nblocks * part : nullptr;
+  cudaError_t e = cudaMemsetAsync(ws, 0, (size_t)nsets * nblocks * part * sizeof(double), st);
+  if (e == cudaSuccess) {
+    bn_reduce_kernel<T, Ty, MODE><<<(unsigned)nblocks, BT, smem, st>>>(
+        (T*)a, a2, zmask, (const Ty*)y, rows, (int)C, l.P, rows_per_block, mean, rstd, ws, (const Ty*)y2, mean2, rstd2, ws2);
+    e = cudaGetLastError();
+  }
+  if (e != cudaSuccess) { set_error("bn reduce launch: %s", cudaGetErrorString(e)); scratch_free(ws, st); return (int)e; }
+  int rc = run_sum_partials_f64(ws, part, sums, part, (int)nblocks, st);
+  if (!rc && sums2) rc = run_sum_partials_f64(ws2, part, sums2, part, (int)nblocks, st);
+  const int rf = scratch_free(ws, st);
+  return rc ? rc : rf;
 }
 
 }  // namespace

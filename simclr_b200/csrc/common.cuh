@@ -1,4 +1,4 @@
-// Shared helpers for the simclr_b200 sm_100a kernels (internal header).
+// Shared helpers for the simclr_b200 sm_90a kernels (internal header).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -47,12 +47,40 @@ inline int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+// Scratch for the partial sums of split reductions: stream-ordered, so it is legal inside CUDA-graph capture
+// (the graph then owns the allocation) and costs no device synchronisation.  Freed memory stays in the pool.
+template <typename T>
+inline int scratch_alloc(T** p, size_t bytes, cudaStream_t st) {
+  static bool pool_kept[64] = {};
+  int dev = 0;
+  SIMCLR_CHECK_CUDA(cudaGetDevice(&dev));
+  if (dev < 64 && !pool_kept[dev]) {
+    cudaMemPool_t pool;
+    uint64_t keep = UINT64_MAX;
+    SIMCLR_CHECK_CUDA(cudaDeviceGetDefaultMemPool(&pool, dev));
+    SIMCLR_CHECK_CUDA(cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep));
+    pool_kept[dev] = true;
+  }
+  SIMCLR_CHECK_CUDA(cudaMallocAsync(reinterpret_cast<void**>(p), bytes, st));
+  return SIMCLR_OK;
+}
+inline int scratch_free(void* p, cudaStream_t st) {
+  SIMCLR_CHECK_CUDA(cudaFreeAsync(p, st));
+  return SIMCLR_OK;
+}
+// dst[i] += the sum of parts[p][i] (part p at ws + p * stride) in an order fixed by `parts` alone: the split reductions of the
+// weight gradients go through it instead of atomics, so that a step computes the same bits every run (defined in tc_conv.cu)
+int run_sum_partials(const float* ws, int64_t stride, float* dst, int64_t n, int parts, cudaStream_t st);
+// the same for the fp64 BatchNorm statistic sums (bn.cu, pool.cu, the fused statistics of the conv epilogues)
+int run_sum_partials_f64(const double* ws, int64_t stride, double* dst, int64_t n, int parts, cudaStream_t st);
+
 
 // ---- device helpers --------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

@@ -1,6 +1,6 @@
 // CUDA-core fp32 convolution engine reading the fp32 HWIO master weights.
 // Deliberately simple (one thread per output element, fp32 FMA): it is the
-// on-device verification engine for the tcgen05 path and the fp32 parity path
+// on-device verification engine for the tensor-core path and the fp32 parity path
 // of the small configs; it is never the default engine.
 // Semantics: tf2/resnet.py:183-208 (stride 1 'SAME', stride>1 FixedPadding +
 // 'VALID'  ==  pad_beg = (k-1)/2 for odd k).

@@ -1,11 +1,11 @@
 // Small kernels around the hot path: supervised-head loss, bias, weight
-// packing for the tcgen05 engine, input preparation (view split + Gaussian
+// packing for the tensor-core engine, input preparation (view split + Gaussian
 // blur + cast + channel pad), error plumbing.
 #include "common.cuh"
 
 namespace simclr {
 
-// Accumulation outputs (BN statistic sums, dW of the tcgen05 wgrad) are normally zeroed by the call that
+// Accumulation outputs (BN statistic sums, dW of the tensor-core wgrad) are normally zeroed by the call that
 // fills them -- one cudaMemsetAsync per call, ~170 per ResNet-50 step.  A caller that zeroes them itself (one
 // memset per step over pooled buffers) switches that off with simclr_set_accumulate_prezeroed(1).
 static bool g_prezeroed = false;
@@ -263,8 +263,8 @@ __global__ void pack_weight_kernel(const float* __restrict__ w, T* __restrict__ 
 
 // ---- input prep ------------------------------------------------------------
 constexpr int MAX_TAPS = 65;
-// outputs per thread along the blurred axis: (2*radius + OUT) / OUT loads per output.  Measured (B200, 224 px, radius 11):
-// the vertical pass gains from 8 (0.52 -> 0.44 ms), the horizontal one loses (0.67 -> 0.87 ms: its lanes are OUT pixels apart)
+// outputs per thread along the blurred axis: (2*radius + OUT) / OUT loads per output.  The vertical pass gains from 8,
+// the horizontal one loses (its lanes are OUT pixels apart)
 constexpr int BLUR_OUT_H = 4, BLUR_OUT_V = 8;
 constexpr int TAP_PAD = BLUR_OUT_V - 1;
 

@@ -383,7 +383,7 @@ int pick_splits(int64_t B, int64_t R, int* tiles_per_split) {
   const int64_t rows = 2 * B, cols = 2 * R * B;
   const int64_t row_blocks = (rows + RB - 1) / RB;
   const int64_t n_tiles = (cols + CT - 1) / CT;
-  int64_t want = (2 * 148 + row_blocks - 1) / row_blocks;
+  int64_t want = (2 * num_sms() + row_blocks - 1) / row_blocks;
   if (want < 1) want = 1;
   if (want > 16) want = 16;
   if (want > n_tiles) want = n_tiles;

@@ -245,8 +245,8 @@ maxpool_bn_bwd_kernel(const T* __restrict__ d, const T* __restrict__ d2, const u
       double t = 0.0;
       for (int r = j; r < 256; r += cv) t += (double)sh_s[r][q];
       const int ch = j * V + (q % V);
-      if (q < V) atomicAdd(&sums[ch], t);
-      else atomicAdd(&sums[C + ch], t * (double)rstd[ch]);
+      if (q < V) sums[(size_t)blockIdx.x * 2 * C + ch] = t;              // this block's partial (summed in block order)
+      else sums[(size_t)blockIdx.x * 2 * C + C + ch] = t * (double)rstd[ch];
     }
   }
 }
@@ -380,8 +380,8 @@ maxpool_bn_bwd_reduce_pooled_bf16_kernel(const __nv_bfloat16* __restrict__ d, co
     double t = 0.0;
     for (int r = j; r < 256; r += cv) t += (double)sh_s[r][q];
     const int ch = j * 8 + (q % 8);
-    if (q < 8) atomicAdd(&sums[ch], t);
-    else atomicAdd(&sums[C + ch], t * (double)rstd[ch]);
+    if (q < 8) sums[(size_t)blockIdx.x * 2 * C + ch] = t;                // this block's partial (summed in block order)
+    else sums[(size_t)blockIdx.x * 2 * C + C + ch] = t * (double)rstd[ch];
   }
 }
 
@@ -632,16 +632,39 @@ static int maxpool_bn_bwd(int phase, const void* d, const void* d2, const uint8_
   cudaStream_t st = (cudaStream_t)stream;
   const int64_t total = N * ((H + 1) / 2) * ((W + 1) / 2) * cv;
   int64_t blocks = (total + 255) / 256;
-  const int64_t cap = (int64_t)num_sms() * (phase == 0 ? 4 : 16);       // phase 0 ends with one atomic per channel per block
+  const int64_t cap = (int64_t)num_sms() * (phase == 0 ? 4 : 16);       // phase 0 ends with one partial per channel per block
   if (blocks > cap) blocks = cap;
   if (phase == 0 && !accumulate_prezeroed()) SIMCLR_CHECK_CUDA(cudaMemsetAsync(sums, 0, 2 * C * sizeof(double), st));
+  // phase 0: every block writes its partial [2][C] to scratch; the partials are added into `sums` in block order
+  double* ws = nullptr;
+  int nparts = 0;
+  if (phase == 0) {
+    nparts = (int)blocks;
+    if (dtype == SIMCLR_BF16 && ysel != nullptr) {
+      const int64_t pb = (N * Ho * Wo * cv + 511) / 512;
+      nparts = (int)(pb > cap ? cap : pb);
+    }
+    int rc = scratch_alloc(&ws, (size_t)nparts * 2 * C * sizeof(double), st);
+    if (rc) return rc;
+    const cudaError_t e = cudaMemsetAsync(ws, 0, (size_t)nparts * 2 * C * sizeof(double), st);
+    if (e != cudaSuccess) { set_error("maxpool_bn_bwd: memset: %s", cudaGetErrorString(e)); scratch_free(ws, st); return (int)e; }
+  }
+  auto finish = [&]() -> int {
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) {
+      set_error("maxpool_bn_bwd: launch: %s", cudaGetErrorString(e));
+      if (ws) scratch_free(ws, st);
+      return (int)e;
+    }
+    if (!ws) return SIMCLR_OK;
+    const int rc = run_sum_partials_f64(ws, 2 * C, sums, 2 * C, nparts, st);
+    const int rf = scratch_free(ws, st);
+    return rc ? rc : rf;
+  };
   if (dtype == SIMCLR_BF16 && phase == 0 && ysel != nullptr) {
     const int64_t ptotal = N * Ho * Wo * cv;
-    int64_t pb = (ptotal + 511) / 512;
-    if (pb > cap) pb = cap;
-    maxpool_bn_bwd_reduce_pooled_bf16_kernel<<<(unsigned)pb, 256, 0, st>>>((const bf16*)d, (const bf16*)d2, (const bf16*)ysel, ptotal, (int)C, mean, rstd, scale, shift, sums);
-    SIMCLR_CHECK_LAUNCH();
-    return SIMCLR_OK;
+    maxpool_bn_bwd_reduce_pooled_bf16_kernel<<<(unsigned)nparts, 256, 0, st>>>((const bf16*)d, (const bf16*)d2, (const bf16*)ysel, ptotal, (int)C, mean, rstd, scale, shift, ws);
+    return finish();
   }
   if (dtype == SIMCLR_BF16 && phase == 1 && N * H * W < (int64_t(1) << 31)) {
 #define MPA(PH, PW) maxpool_bn_bwd_apply_bf16_kernel<PH, PW><<<(unsigned)blocks, 256, 0, st>>>((const bf16*)d, (const bf16*)d2, argmax, (const bf16*)y, (bf16*)dy, total, (int)H, (int)W, (int)C, (int)Ho, (int)Wo, scale, shift, coef)
@@ -650,13 +673,12 @@ static int maxpool_bn_bwd(int phase, const void* d, const void* d2, const uint8_
     SIMCLR_CHECK_LAUNCH();
     return SIMCLR_OK;
   }
-#define MPB(T, PH) maxpool_bn_bwd_kernel<T, PH><<<(unsigned)blocks, 256, 0, st>>>((const T*)d, (const T*)d2, argmax, (const T*)y, (T*)dy, total, (int)H, (int)W, (int)C, (int)Ho, (int)Wo, pbh, pbw, mean, rstd, scale, shift, coef, sums)
+#define MPB(T, PH) maxpool_bn_bwd_kernel<T, PH><<<(unsigned)blocks, 256, 0, st>>>((const T*)d, (const T*)d2, argmax, (const T*)y, (T*)dy, total, (int)H, (int)W, (int)C, (int)Ho, (int)Wo, pbh, pbw, mean, rstd, scale, shift, coef, ws)
   if (dtype == SIMCLR_F32) { if (phase == 0) MPB(float, 0); else MPB(float, 1); }
   else if (dtype == SIMCLR_BF16) { if (phase == 0) MPB(bf16, 0); else MPB(bf16, 1); }
-  else { set_error("maxpool_bn_bwd: unknown dtype"); return SIMCLR_ERR_INVALID_ARG; }
+  else { set_error("maxpool_bn_bwd: unknown dtype"); if (ws) scratch_free(ws, st); return SIMCLR_ERR_INVALID_ARG; }
 #undef MPB
-  SIMCLR_CHECK_LAUNCH();
-  return SIMCLR_OK;
+  return finish();
 }
 
 int simclr_maxpool_bn_bwd_reduce(const void* d, const void* d2, const uint8_t* argmax, const void* y,

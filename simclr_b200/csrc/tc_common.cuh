@@ -1,5 +1,5 @@
-// sm_100a building blocks for the tcgen05 engine: mbarrier, TMA, TMEM and UMMA
-// wrappers (inline PTX), smem/instruction descriptors, host-side tensor maps.
+// sm_90a building blocks for the tensor-core engine: mbarrier, TMA and wgmma
+// wrappers (inline PTX), shared-memory descriptors, host-side tensor maps.
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
@@ -26,14 +26,15 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                : "memory");
 }
-// Spin on a phase parity.  A bounded spin turns a protocol bug into a trap (the
-// launch fails with an error) instead of a hung GPU.
+// Spin on a phase parity.  A bounded spin turns a protocol bug into a trap (the launch fails with an
+// error) instead of a hung GPU.  No function call (printf) may sit here: the consumers wait inside their
+// wgmma pipelines, and a call there makes ptxas serialise every wgmma of the kernel.
 __device__ __forceinline__ uint64_t global_timer_ns() {
   uint64_t t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
   return t;
 }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int tag = 0) {
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   const uint32_t addr = smem_u32(bar);
   uint32_t ok = 0;
   uint64_t t0 = 0;
@@ -52,14 +53,11 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int ta
     if ((++spins & 0xFF) == 0) {
       const uint64_t now = global_timer_ns();
       if (t0 == 0) t0 = now;
-      else if (now - t0 > 4000000000ull) {     // 4 s: a protocol bug, not a long kernel
-        printf("simclr_b200: mbarrier timeout tag=%d block=%d thread=%d parity=%u\n", tag, blockIdx.x, threadIdx.x, parity);
-        __trap();
-      }
+      else if (now - t0 > 4000000000ull) __trap();     // 4 s: a protocol bug, not a long kernel
     }
   }
 }
-// generic-proxy smem writes -> visible to the async proxy (UMMA / TMA reads)
+// generic-proxy smem writes -> visible to the async proxy (wgmma / TMA reads)
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------
@@ -74,24 +72,24 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
       ::"r"(smem_u32(smem_dst)), "l"((uint64_t)tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-// packed fp32 pairs (sm_100 FADD2 / FFMA2): halves the instruction count of the statistics loops
+// fp32 pairs kept in one 64-bit register (the statistics loops' running sums)
 __device__ __forceinline__ uint64_t f2_pack(float lo, float hi) {
   uint64_t r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r;
 }
 __device__ __forceinline__ void f2_unpack(uint64_t v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
 __device__ __forceinline__ uint64_t f2_add(uint64_t a, uint64_t b) {
-  uint64_t r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r;
+  float a0, a1, b0, b1; f2_unpack(a, a0, a1); f2_unpack(b, b0, b1); return f2_pack(a0 + b0, a1 + b1);
 }
 __device__ __forceinline__ uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r;
+  float a0, a1, b0, b1, c0, c1; f2_unpack(a, a0, a1); f2_unpack(b, b0, b1); f2_unpack(c, c0, c1);
+  return f2_pack(fmaf(a0, b0, c0), fmaf(a1, b1, c1));
 }
 
 // im2col-mode load from an NHWC tensor (rank 4: {C, W, H, N}): `pixels-per-column` consecutive base
 // pixels starting at (w, h, n) -- walking W, then H, then N inside the map's bounding box with its
 // traversal stride -- each displaced by the filter offset (off_w, off_h); `channels-per-pixel`
 // channels from c.  Pixels outside the image (padding, n >= N) read as zero.  The smem image is the
-// same [pixel][128 B] 128B-swizzled tile a tiled 2-D box produces.  (Semantics pinned on sm_100a
-// with scripts/probe_im2col.cu.)
+// same [pixel][128 B] 128B-swizzled tile a tiled 2-D box produces.
 __device__ __forceinline__ void tma_load_im2col(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, int c, int w,
                                                 int h, int n, int off_w, int off_h) {
   const uint16_t ow = (uint16_t)off_w, oh = (uint16_t)off_h;
@@ -139,104 +137,167 @@ __device__ __forceinline__ void named_barrier_sync(int id, int threads) {
 }
 
 // ---------------------------------------------------------------------------
-// TMEM + tcgen05
+// wgmma (sm_90a): D[registers of the issuing warpgroup] (+)= A[smem] * B[smem]
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]; single thread issues on behalf of the CTA.
-template <bool TF32>
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if (TF32) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n}\n"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+// A 128-row tile is two m64 halves; D of one half, m64nNk16 with fp32 accumulators, is N/2 registers per thread:
+// d[4*i + v] holds row 16*(warp % 4) + lane/4 + 8*(v >> 1), column 8*i + 2*(lane % 4) + (v & 1).
+template <int N, bool TF32, bool A_MN, bool B_MN> struct Wgmma;
+template <> struct Wgmma<32, false, false, false> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "l"(da), "l"(db), "r"(acc));
   }
+};
+
+template <> struct Wgmma<32, false, true, true> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 1, 1;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+                 : "l"(da), "l"(db), "r"(acc));
+  }
+};
+
+template <> struct Wgmma<64, false, false, false> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(da), "l"(db), "r"(acc));
+  }
+};
+
+template <> struct Wgmma<64, false, true, true> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 1, 1;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(da), "l"(db), "r"(acc));
+  }
+};
+
+template <> struct Wgmma<128, false, false, false> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(da), "l"(db), "r"(acc));
+  }
+};
+
+template <> struct Wgmma<128, false, true, true> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 1, 1;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(da), "l"(db), "r"(acc));
+  }
+};
+
+template <> struct Wgmma<64, true, false, false> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+                 : "l"(da), "l"(db), "r"(acc));
+  }
+};
+
+template <> struct Wgmma<128, true, false, false> {
+  static __device__ __forceinline__ void mma(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+                 "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n}\n"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+                 : "l"(da), "l"(db), "r"(acc));
+  }
+};
+
+// D (+)= A * B for one m64 half; `acc` == 0 overwrites D (first K step of a tile)
+template <int N, bool TF32, bool A_MN, bool B_MN>
+__device__ __forceinline__ void wgmma(float* d, uint64_t da, uint64_t db, uint32_t acc) {
+  Wgmma<N, TF32, A_MN, B_MN>::mma(d, da, db, acc);
 }
-// mbarrier arrives when all tcgen05 ops previously issued by this thread are done.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+// orders register / shared-memory accesses of the warpgroup before the wgmmas that follow
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// at most N committed groups still in flight; the accumulators are named so that they are not read early
+template <int N, int H, int R>
+__device__ __forceinline__ void wgmma_wait(float (&d)[H][R]) {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+#pragma unroll
+  for (int h = 0; h < H; ++h)
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[h][i])::"memory");
 }
-// 32 lanes x 32 consecutive fp32 columns: thread t of the warp gets row (lane_base + t).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// Row of the 128-row tile that accumulator registers 4*i + 2*rp (+1) of half h hold (rp: first or second row of
+// the thread within its 16-row slice), for a warpgroup made of warps 0-3 of its own 128 threads.
+__device__ __forceinline__ int frag_row(int h, int rp) {
+  return 64 * h + 16 * ((threadIdx.x >> 5) & 3) + ((threadIdx.x & 31) >> 2) + 8 * rp;
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------
-// Descriptors (bit layouts: cute/arch/mma_sm100_desc.hpp)
+// Descriptors (sm_90 wgmma layout)
 // ---------------------------------------------------------------------------
 // Shared-memory matrix descriptor, 128B swizzle.  K-major tiles: rows of 128 B,
 // 8-row groups SBO bytes apart (LBO unused, encoded as 1).  MN-major tiles:
 // 128-B rows along MN, 8-row (K) groups SBO apart, MN atoms LBO apart.
-__device__ __forceinline__ uint64_t smem_desc_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);            // start address, bits [0,14)
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;   // leading byte offset, bits [16,30)
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;   // stride byte offset, bits [32,46)
-  d |= (uint64_t)1 << 46;                             // descriptor version 1 (sm_100)
-  d |= (uint64_t)2 << 61;                             // SWIZZLE_128B
-  return d;
-}
-// The same descriptor from its two 32-bit halves: only the 14-bit start-address field (bytes >> 4) changes between
-// the MMAs of a tile, so the issuing warp keeps `lo` as a running 32-bit value (one add per MMA, computed
-// warp-uniformly so that it lives in a uniform register) instead of rebuilding 64 bits from an address.
+// Only the 14-bit start-address field (bytes >> 4) changes between the MMAs of a tile, so the issuing warpgroup
+// keeps the low word as a running 32-bit value instead of rebuilding 64 bits from an address.
 __host__ __device__ constexpr uint32_t desc_hi_sw128(uint32_t sbo_bytes) {
-  return ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 14) | (2u << 29);
+  return ((sbo_bytes >> 4) & 0x3FFFu) | (1u << 30);                 // layout type 1 (SWIZZLE_128B), bits 62-63
 }
+// no swizzle ("interleaved" 8-row x 16-byte core matrices)
+__host__ __device__ constexpr uint32_t desc_hi_none(uint32_t sbo_bytes) { return (sbo_bytes >> 4) & 0x3FFFu; }
 __device__ __forceinline__ uint32_t desc_lo(uint32_t saddr, uint32_t lbo_bytes) {
   return ((saddr & 0x3FFFFu) >> 4) | (((lbo_bytes >> 4) & 0x3FFFu) << 16);
 }
 __device__ __forceinline__ uint64_t desc_pack(uint32_t lo, uint32_t hi) {
   uint64_t d; asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "r"(lo), "r"(hi)); return d;
 }
-// one lane of a converged warp (the form the compiler recognises for single-thread tcgen05 issue)
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n.reg .pred p;\nelect.sync _|p, 0xffffffff;\nselp.u32 %0, 1, 0, p;\n}\n" : "=r"(pred));
-  return pred != 0;
-}
 // value of lane 0, provably warp-uniform for the compiler
 __device__ __forceinline__ uint32_t uniform_u32(uint32_t v) { return __shfl_sync(0xffffffffu, v, 0); }
-
-// Instruction descriptor for kind::f16 (bf16) / kind::tf32, fp32 accumulate.
-__host__ __device__ constexpr uint32_t make_idesc(bool tf32, int M, int N, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4)                               // c_format = F32
-         | ((tf32 ? 2u : 1u) << 7)               // a_format: BF16=1, TF32=2
-         | ((tf32 ? 2u : 1u) << 10)              // b_format
-         | ((a_mn_major ? 1u : 0u) << 15) | ((b_mn_major ? 1u : 0u) << 16)
-         | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
 
 // byte offset of 16-byte chunk j of row r inside a [rows][128 B] SWIZZLE_128B tile
 __device__ __forceinline__ uint32_t sw128_offset(int row, int chunk) {
   return (uint32_t)(row * 128 + ((chunk ^ (row & 7)) << 4));
+}
+
+// Accumulator columns [8*i0, 8*i0 + 128 / sizeof(To)) of a 128-row tile (both halves) -> [128 rows][128 B]
+// 128B-swizzled staging tile at shared address `tile`, converted to To; rows with ok[h][rp] false are stored as zeros.
+template <typename To, int NF>
+__device__ __forceinline__ void stage_frag(uint32_t tile, const float (&acc)[2][NF], int i0, const bool (&ok)[2][2]) {
+  constexpr int NI = 128 / (int)sizeof(To) / 8;      // 8-column groups per 128-byte row
+  const int q = threadIdx.x & 3;
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int rp = 0; rp < 2; ++rp) {
+      const int row = frag_row(h, rp);
+#pragma unroll
+      for (int ii = 0; ii < NI; ++ii) {
+        float a = acc[h][4 * (i0 + ii) + 2 * rp], b = acc[h][4 * (i0 + ii) + 2 * rp + 1];
+        if (!ok[h][rp]) { a = 0.f; b = 0.f; }
+        if (sizeof(To) == 2) {
+          __nv_bfloat162 hh = __floats2bfloat162_rn(a, b);
+          asm volatile("st.shared.u32 [%0], %1;" ::"r"(tile + sw128_offset(row, ii) + 4 * q), "r"(*reinterpret_cast<uint32_t*>(&hh)) : "memory");
+        } else {
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(tile + sw128_offset(row, 2 * ii + (q >> 1)) + 8 * (q & 1)), "f"(a), "f"(b) : "memory");
+        }
+      }
+    }
+}
+// the 32 fp32 values of `row` from a [128 rows][128 B] 128B-swizzled staging tile
+__device__ __forceinline__ void load_row32(const uint8_t* tile, int row, uint32_t* r) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const uint4 v = *reinterpret_cast<const uint4*>(tile + sw128_offset(row, j));
+    r[4 * j] = v.x; r[4 * j + 1] = v.y; r[4 * j + 2] = v.z; r[4 * j + 3] = v.w;
+  }
 }
 
 // Division by a runtime constant (CUTLASS FastDivmod scheme; n < 2^31).

@@ -1,14 +1,14 @@
-// tcgen05 implicit-GEMM engine for conv fprop / dgrad / wgrad and the dense
+// wgmma implicit-GEMM engine for conv fprop / dgrad / wgrad and the dense
 // layers (tf2/resnet.py:183-208, tf2/model.py:143-151).
 //
 // One persistent, warp-specialised kernel per GEMM flavour:
-//   warps 0-3  epilogue     TMEM -> registers (tcgen05.ld) -> global
-//   warp  4    MMA issuer   one elected lane issues tcgen05.mma, accumulators in TMEM
-//   warp  5    TMA producer weights / dY tiles (and activations for 1x1 stride-1)
-//   warps 6-9  gather       im2col rows of NHWC activations -> 128B-swizzled smem
-// Pipelines: smem full/empty mbarriers (producers <-> MMA) and a double-buffered
-// TMEM accumulator (MMA <-> epilogue), so the epilogue of tile i overlaps the
-// main loop of tile i+1.  Tiles: 128 (TMEM lanes) x BN x 128 bytes of K per stage.
+//   warps 0-3  consumer     one warpgroup issues wgmma (two m64 halves per 128-row tile, fp32
+//                           accumulators in registers) and runs the epilogue -> global
+//   warp  4    TMA producer weights / dY tiles (and activations for 1x1 stride-1)
+//   warps 5-8  gather       im2col rows of NHWC activations -> 128B-swizzled smem
+// Pipeline: smem full/empty mbarriers (producers <-> consumer); the producers run ahead into
+// the next tile while the consumer drains the accumulators.  Tiles: 128 x BN x 128 bytes of K
+// per stage, BN <= 128 (a 128 x 128 fp32 accumulator is 128 registers per consumer thread).
 #include "tc_common.cuh"
 
 namespace simclr {
@@ -17,35 +17,32 @@ namespace {
 
 constexpr int A_STAGE_BYTES = 128 * 128;     // 128 rows x 128 B
 constexpr int PIPE_BYTES = 192 * 1024;
-constexpr int EPI_THREADS = 128;
-constexpr int GATHER_THREADS = 256;   // 8 gather warps: two per scheduler hide each other's address arithmetic
-constexpr int STATS_THREADS = 128;    // 4 statistics warps (TMA-fed fprop)
+constexpr int EPI_THREADS = 128;     // the consumer warpgroup
+constexpr int AUX_T0 = 160;          // first thread after the consumer warpgroup and the TMA warp
+constexpr int GATHER_THREADS = 128;  // 4 gather warps (the consumer's accumulators need the register file)
+constexpr int STATS_THREADS = 128;   // 4 statistics warps (TMA-fed fprop)
 constexpr int GROWS = GATHER_THREADS / 8;   // tile rows covered by one pass of the gather threads (8 threads per row)
 constexpr int GPT = 128 / GROWS;            // 16-byte pieces per gather thread per stage
-constexpr int igemm_threads(bool a_tma, bool stats) { return a_tma ? (stats ? 192 + STATS_THREADS : 192) : 192 + GATHER_THREADS; }
-constexpr int wgrad_threads(bool a_tma) { return a_tma ? 192 : 192 + GATHER_THREADS; }
+constexpr int igemm_threads(bool a_tma, bool stats) { return a_tma ? (stats ? AUX_T0 + STATS_THREADS : AUX_T0) : AUX_T0 + GATHER_THREADS; }
+constexpr int wgrad_threads(bool a_tma) { return a_tma ? AUX_T0 : AUX_T0 + GATHER_THREADS; }
+// A CTA's warps are spread over the SM's four 16K-register sub-partitions: with the 9 warps of the gather-fed kernels
+// one sub-partition holds 3, which caps a thread at 168 registers, and their 128-column accumulators spill a little.
 
 template <int BN> struct Tile {
   static constexpr int B_STAGE_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
   static constexpr int STAGES = PIPE_BYTES / STAGE_BYTES;
-  static constexpr int TMEM_COLS = 2 * BN < 32 ? 32 : 2 * BN;   // double-buffered accumulator (power of 2)
   static constexpr int EPI_BYTES = 2 * A_STAGE_BYTES;           // two [128 rows][128 B] store staging tiles
   static constexpr int GATHER_DEPTH = STAGES > 4 ? 4 : STAGES - 1;   // cp.async groups in flight per thread
   static constexpr size_t SMEM_BYTES = 1024 /*align*/ + (size_t)STAGES * STAGE_BYTES + EPI_BYTES + 256 /*barriers*/;
 };
 
-// wgrad work item: MT x 128 k-rows (MT accumulators sharing every dY tile).  MT = 2 halves the dY bytes that
-// cross L2 -> SM per MMA (wide layers are bound by that traffic, not by the tensor pipe); its 2 x BN fp32
-// accumulator columns fill TMEM for BN = 256, so the accumulators are single-buffered (items are long
-// pixel loops: the un-overlapped epilogue is a few percent).
-template <int BN, int MT> struct WTile {
-  static constexpr int A_BYTES = MT * A_STAGE_BYTES;
+// wgrad work item: 128 k-rows x BN output channels x a run of pixel blocks
+template <int BN> struct WTile {
+  static constexpr int A_BYTES = A_STAGE_BYTES;
   static constexpr int B_STAGE_BYTES = BN * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_STAGE_BYTES;
   static constexpr int STAGES = PIPE_BYTES / STAGE_BYTES;
-  static constexpr int NACC = MT == 1 ? 2 : 1;                       // accumulator sets in flight
-  static constexpr int TMEM_COLS = NACC * MT * BN < 32 ? 32 : NACC * MT * BN;
   static constexpr int GATHER_DEPTH = STAGES > 4 ? 4 : STAGES - 1;
   static constexpr size_t SMEM_BYTES = 1024 + (size_t)STAGES * STAGE_BYTES + 2 * A_STAGE_BYTES + 256;
 };
@@ -64,6 +61,8 @@ struct Geom {
   int tiles_m, tiles_n;
   // wgrad only
   int Cin, Cout, splits, kb_per_split;
+  float* ws;           // splits > 1: per-split partials ([splits][ws_rows][Cout] or [splits][dW]), summed in split order
+  long long ws_stride; // floats per split partial
   // strided-dgrad parity classes: taps from a table, output rows scattered with stride `os`
   int use_tab, cblocks;
   int P, Q;            // GEMM-row pixel grid (wgrad: incremental pixel walk)
@@ -74,7 +73,6 @@ struct Geom {
   // TMA im2col feed of the gathered operand: base pixel of GEMM row (n, p, q) is
   // (q*stride + im_base, p*stride + im_base); the tap goes into the instruction's filter offsets
   int im2col, im_base, im_nimg;
-  int wg_mt;           // wgrad: 128-row k tiles per work item (1 or 2)
   int accum;           // fp32 outputs only: add into `out` (TMA reduce-add / atomics) instead of storing (tc3 passes)
 };
 
@@ -102,10 +100,6 @@ __device__ __forceinline__ TapRef decode_tap(const Geom& g, uint32_t tap) {
     t.dr = g.tap_sign * (int)r; t.ds = g.tap_sign * (int)s;
   }
   return t;
-}
-
-__device__ __forceinline__ void sts16(uint32_t saddr, uint4 v) {
-  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 
 template <typename To>
@@ -147,7 +141,7 @@ __device__ __forceinline__ void warp_arrive(uint64_t* bar) {
 }
 
 struct SmemCtl {
-  uint64_t* full; uint64_t* empty; uint64_t* tmem_full; uint64_t* tmem_empty; uint32_t* tmem_ptr;
+  uint64_t* full; uint64_t* empty;
   uint64_t* sfull; uint64_t* sfree;   // staging tile handed to / returned by the statistics warps
   uint8_t* epi;     // 2 x [128][128 B] staging tiles for the TMA-store epilogue
 };
@@ -156,9 +150,8 @@ __device__ __forceinline__ SmemCtl carve(uint8_t* base, int stage_bytes) {
   SmemCtl c;
   c.epi = base + (size_t)STAGES * stage_bytes;
   uint64_t* b = reinterpret_cast<uint64_t*>(c.epi + 2 * A_STAGE_BYTES);
-  c.full = b; c.empty = b + STAGES; c.tmem_full = b + 2 * STAGES; c.tmem_empty = b + 2 * STAGES + 2;
-  c.sfull = b + 2 * STAGES + 4; c.sfree = b + 2 * STAGES + 6;
-  c.tmem_ptr = reinterpret_cast<uint32_t*>(b + 2 * STAGES + 8);
+  c.full = b; c.empty = b + STAGES;
+  c.sfull = b + 2 * STAGES; c.sfree = b + 2 * STAGES + 2;
   return c;
 }
 
@@ -174,7 +167,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
   constexpr bool TF32 = Elt<T>::TF32;
   constexpr int KBE = Elt<T>::KBE;
   constexpr int CH = Elt<T>::CH;
-  constexpr uint32_t IDESC = make_idesc(TF32, 128, BN, false, false);
+  constexpr int NF = BN / 2;                          // accumulator registers per thread and m64 half
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -184,159 +177,118 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&ctl.full[s], A_TMA ? 1 : 1 + GATHER_THREADS / 32);
-      mbar_init(&ctl.empty[s], 1);
+      mbar_init(&ctl.empty[s], EPI_THREADS / 32);
     }
-    for (int a = 0; a < 2; ++a) { mbar_init(&ctl.tmem_full[a], 1); mbar_init(&ctl.tmem_empty[a], EPI_THREADS / 32); }
     for (int a = 0; a < 2; ++a) { mbar_init(&ctl.sfull[a], 1); mbar_init(&ctl.sfree[a], STATS_THREADS / 32); }
     fence_barrier_init();
   }
-  if (warp == 5 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     tma_prefetch_desc(&tmap_b);
     if (A_TMA) tma_prefetch_desc(&tmap_a);
     if (TMA_EPI) tma_prefetch_desc(&tmap_out);
   }
-  // With TMA-fed activations warps 6-9 have no gather to do: they take the BatchNorm statistics off the
+  // With TMA-fed activations warps 5-8 have no gather to do: they take the BatchNorm statistics off the
   // epilogue's critical path (short-K 1x1 layers are epilogue-bound).
   constexpr bool STATS_WARPS = STATS && A_TMA;
   constexpr int BOX_COLS = 128 / (int)sizeof(To);     // 64 (bf16) / 32 (fp32) output columns per staged tile
   constexpr int BOXES = BN / BOX_COLS;
   constexpr int CPC = 16 / (int)sizeof(To);           // columns per 16-byte chunk: 8 (bf16) / 4 (fp32)
-  if (warp == 4) tmem_alloc(ctl.tmem_ptr, TL::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *ctl.tmem_ptr;
   const int num_tiles = g.tiles_m * g.tiles_n;
 
   if (warp < 4) {
-    // ------------------------------ epilogue ------------------------------
-    int as = 0; uint32_t aphase = 0;
+    // ------------------------------ consumer: MMA + epilogue ------------------------------
+    // Descriptor low words are running 32-bit sums (one uniform add per MMA); a stage is handed back to the
+    // producers once the wgmma group after it has been issued and it has retired (one group in flight).
+    constexpr uint32_t HI = desc_hi_sw128(1024);
+    const uint32_t smem_lo = uniform_u32(desc_lo(smem_u32(smem), 16));
+    const bool all_rows[2][2] = {{true, true}, {true, true}};   // rows >= M hold exact zeros / are clipped
+    float acc[2][NF];
+    Pipe pp{0, 0};
     To* out = reinterpret_cast<To*>(g.out);
-    if (TMA_EPI) {
-      // TMEM -> registers -> 128B-swizzled smem tile [128 rows][128 B] -> TMA store (coalesced,
-      // rows >= M and columns >= n_out clipped by the tensor map).  Two staging tiles alternate.
-      constexpr int LDS_PER_BOX = BOX_COLS / 32;
-      uint32_t box_ctr = 0;                                // counts staged ("live") boxes only
-      const int row = warp * 32 + lane;
-      // fused BatchNorm statistics (tf2/resnet.py:50-72): per-column sum / sum of squares of the
-      // *stored* (rounded) outputs, accumulated in registers over all tiles of this CTA (the host
-      // makes gridDim a multiple of tiles_n so a CTA keeps one column block) and flushed once.
-      // Thread t owns 16-byte chunk (t & 7) -- CPC consecutive columns -- of rows (t >> 3)*8 .. +7 of
-      // every staged tile: 8 conflict-free LDS.128 per box, partial sums kept in registers.
-      const int sj = threadIdx.x & 7, srg = threadIdx.x >> 3;
-      float st_sum[BOXES][CPC], st_sq[BOXES][CPC];
+    uint32_t box_ctr = 0;                                // counts staged ("live") boxes only
+    // fused BatchNorm statistics (tf2/resnet.py:50-72): per-column sum / sum of squares of the
+    // *stored* (rounded) outputs, accumulated in registers over all tiles of this CTA (the host
+    // makes gridDim a multiple of tiles_n so a CTA keeps one column block) and flushed once.
+    // Thread t owns 16-byte chunk (t & 7) -- CPC consecutive columns -- of rows (t >> 3)*8 .. +7 of
+    // every staged tile: 8 conflict-free LDS.128 per box, partial sums kept in registers.
+    const int sj = threadIdx.x & 7, srg = threadIdx.x >> 3;
+    float st_sum[BOXES][CPC], st_sq[BOXES][CPC];
 #pragma unroll
-      for (int b = 0; b < BOXES; ++b)
+    for (int b = 0; b < BOXES; ++b)
 #pragma unroll
-        for (int c = 0; c < CPC; ++c) { st_sum[b][c] = 0.f; st_sq[b][c] = 0.f; }
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int tm = tile / g.tiles_n, tn = tile - tm * g.tiles_n;
-        mbar_wait(&ctl.tmem_full[as], aphase, 10);
-        tc_fence_after();
-        const uint32_t tbase = tmem_base + (uint32_t)(as * BN) + ((uint32_t)(warp * 32) << 16);
-#pragma unroll 1
+      for (int c = 0; c < CPC; ++c) { st_sum[b][c] = 0.f; st_sq[b][c] = 0.f; }
+    const bool vec_ok = ((reinterpret_cast<uintptr_t>(out) & 15) == 0) && ((g.ldc * (int)sizeof(To)) % 16 == 0);
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int tm = tile / g.tiles_n, tn = tile - tm * g.tiles_n;
+      int prev = 0;
+      for (int kb = 0; kb < g.num_kb; ++kb) {
+        mbar_wait(&ctl.full[pp.stage], pp.phase);
+        const uint32_t a_lo = smem_lo + (uint32_t)pp.stage * (TL::STAGE_BYTES >> 4);
+        const uint32_t b_lo = a_lo + (A_STAGE_BYTES >> 4);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k)          // 4 x (32 bytes of K) per stage
+#pragma unroll
+          for (int h = 0; h < 2; ++h)        // rows 64h .. 64h + 63: 64 rows x 128 B further
+            wgmma<BN, TF32, false, false>(acc[h], desc_pack(a_lo + h * (64 * 128 >> 4) + 2 * k, HI), desc_pack(b_lo + 2 * k, HI),
+                                          (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        if (kb > 0) { wgmma_wait<1>(); warp_arrive(&ctl.empty[prev]); }
+        prev = pp.stage;
+        advance<STAGES>(pp);
+      }
+      wgmma_wait<0>(acc);
+      warp_arrive(&ctl.empty[prev]);
+
+      if (TMA_EPI) {
+        // registers -> 128B-swizzled smem tile [128 rows][128 B] -> TMA store (coalesced, rows >= M and
+        // columns >= n_out clipped by the tensor map).  Two staging tiles alternate.
+#pragma unroll
         for (int b = 0; b < BOXES; ++b) {
           uint8_t* stage = ctl.epi + (box_ctr & 1) * A_STAGE_BYTES;
           const int n0 = tn * BN + b * BOX_COLS;
-          const bool live = n0 < g.n_out;                 // uniform across the CTA
-          if (live) {
-            if (threadIdx.x == 0) {
-              tma_store_wait_read<1>();   // the store issued two boxes ago has read its tile
-              if (STATS_WARPS) mbar_wait(&ctl.sfree[box_ctr & 1], ((box_ctr >> 1) & 1) ^ 1, 11);   // ... and so have the stats warps
-            }
-            named_barrier_sync(1, EPI_THREADS);
+          if (n0 >= g.n_out) continue;                     // uniform across the CTA
+          if (threadIdx.x == 0) {
+            tma_store_wait_read<1>();   // the store issued two boxes ago has read its tile
+            if (STATS_WARPS) mbar_wait(&ctl.sfree[box_ctr & 1], ((box_ctr >> 1) & 1) ^ 1);   // ... and so have the stats warps
           }
-          const uint32_t srow = smem_u32(stage);
+          named_barrier_sync(1, EPI_THREADS);
+          stage_frag<To>(smem_u32(stage), acc, b * BOX_COLS / 8, all_rows);
+          fence_proxy_async();
+          named_barrier_sync(1, EPI_THREADS);
+          if (threadIdx.x == 0) {
+            if (sizeof(To) == 4 && g.accum) tma_reduce_add_2d(&tmap_out, stage, n0, tm * 128);
+            else tma_store_2d(&tmap_out, stage, n0, tm * 128);
+            tma_store_commit();
+            if (STATS_WARPS) mbar_arrive(&ctl.sfull[box_ctr & 1]);
+          }
+          if (STATS && !STATS_WARPS) {
+            float a0[CPC], a1[CPC];
 #pragma unroll
-          for (int h = 0; h < LDS_PER_BOX; ++h) {
-            uint32_t acc[32];
-            tmem_ld32(tbase + b * BOX_COLS + h * 32, acc);
-            tmem_ld_wait();
-            if (live) {
+            for (int c = 0; c < CPC; ++c) { a0[c] = 0.f; a1[c] = 0.f; }
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {                 // rows srg*8 + i (rows >= M hold exact zeros)
+              const uint4 raw = *reinterpret_cast<const uint4*>(stage + (srg * 8 + i) * 128 + ((sj ^ i) << 4));
+              float v[CPC];
               if (sizeof(To) == 2) {
+                const uint32_t w[4] = {raw.x, raw.y, raw.z, raw.w};
 #pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  uint32_t w[4];
-#pragma unroll
-                  for (int e = 0; e < 4; ++e) {
-                    __nv_bfloat162 hh = __floats2bfloat162_rn(__uint_as_float(acc[8 * q + 2 * e]), __uint_as_float(acc[8 * q + 2 * e + 1]));
-                    w[e] = *reinterpret_cast<uint32_t*>(&hh);
-                  }
-                  sts16(srow + sw128_offset(row, h * 4 + q), make_uint4(w[0], w[1], w[2], w[3]));
-                }
+                for (int e = 0; e < 4; ++e) { v[(2 * e) % CPC] = __uint_as_float(w[e] << 16); v[(2 * e + 1) % CPC] = __uint_as_float(w[e] & 0xffff0000u); }
               } else {
-#pragma unroll
-                for (int q = 0; q < 8; ++q)
-                  sts16(srow + sw128_offset(row, q), make_uint4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]));
-              }
-            }
-          }
-          if (b == BOXES - 1) { tc_fence_before(); warp_arrive(&ctl.tmem_empty[as]); }   // accumulator drained
-          if (live) {
-            fence_proxy_async();
-            named_barrier_sync(1, EPI_THREADS);
-            if (threadIdx.x == 0) {
-              if (sizeof(To) == 4 && g.accum) tma_reduce_add_2d(&tmap_out, stage, n0, tm * 128);
-              else tma_store_2d(&tmap_out, stage, n0, tm * 128);
-              tma_store_commit();
-              if (STATS_WARPS) mbar_arrive(&ctl.sfull[box_ctr & 1]);
-            }
-            if (STATS && !STATS_WARPS) {
-              float a0[CPC], a1[CPC];
-#pragma unroll
-              for (int c = 0; c < CPC; ++c) { a0[c] = 0.f; a1[c] = 0.f; }
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {                 // rows srg*8 + i (rows >= M hold exact zeros)
-                const uint4 raw = *reinterpret_cast<const uint4*>(stage + (srg * 8 + i) * 128 + ((sj ^ i) << 4));
-                float v[CPC];
-                if (sizeof(To) == 2) {
-                  const uint32_t w[4] = {raw.x, raw.y, raw.z, raw.w};
-#pragma unroll
-                  for (int e = 0; e < 4; ++e) { v[(2 * e) % CPC] = __uint_as_float(w[e] << 16); v[(2 * e + 1) % CPC] = __uint_as_float(w[e] & 0xffff0000u); }
-                } else {
-                  v[0] = __uint_as_float(raw.x); v[1] = __uint_as_float(raw.y); v[2 % CPC] = __uint_as_float(raw.z); v[3 % CPC] = __uint_as_float(raw.w);
-                }
-#pragma unroll
-                for (int c = 0; c < CPC; ++c) { a0[c] += v[c]; a1[c] = fmaf(v[c], v[c], a1[c]); }
+                v[0] = __uint_as_float(raw.x); v[1] = __uint_as_float(raw.y); v[2 % CPC] = __uint_as_float(raw.z); v[3 % CPC] = __uint_as_float(raw.w);
               }
 #pragma unroll
-              for (int bb = 0; bb < BOXES; ++bb)
-                if (bb == b) {
-#pragma unroll
-                  for (int c = 0; c < CPC; ++c) { st_sum[bb][c] += a0[c]; st_sq[bb][c] += a1[c]; }
-                }
+              for (int c = 0; c < CPC; ++c) { a0[c] += v[c]; a1[c] = fmaf(v[c], v[c], a1[c]); }
             }
-            ++box_ctr;
-          }
-        }
-        as ^= 1; if (as == 0) aphase ^= 1;
-      }
-      if (STATS && !STATS_WARPS) {
-        const int tn0 = blockIdx.x % g.tiles_n;            // constant for this CTA (gridDim % tiles_n == 0)
 #pragma unroll
-        for (int b = 0; b < BOXES; ++b) {
-#pragma unroll
-          for (int c = 0; c < CPC; ++c) {
-            // fold the 4 row groups of the warp (lane >> 3) onto lanes 0-7
-            float s0 = st_sum[b][c], s1 = st_sq[b][c];
-            s0 += __shfl_xor_sync(0xffffffffu, s0, 8);  s1 += __shfl_xor_sync(0xffffffffu, s1, 8);
-            s0 += __shfl_xor_sync(0xffffffffu, s0, 16); s1 += __shfl_xor_sync(0xffffffffu, s1, 16);
-            const int col = tn0 * BN + b * BOX_COLS + sj * CPC + c;
-            if (lane < 8 && col < g.n_out && (int)blockIdx.x < num_tiles) {
-              atomicAdd(bn_sums + col, (double)s0);
-              atomicAdd(bn_sums + g.n_out + col, (double)s1);
-            }
+            for (int c = 0; c < CPC; ++c) { st_sum[b][c] += a0[c]; st_sq[b][c] += a1[c]; }
           }
+          ++box_ctr;
         }
-      }
-      if (threadIdx.x == 0) tma_store_wait_all<0>();
-    } else {
-      const bool vec_ok = ((reinterpret_cast<uintptr_t>(out) & 15) == 0) && ((g.ldc * (int)sizeof(To)) % 16 == 0);
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int tm = tile / g.tiles_n, tn = tile - tm * g.tiles_n;
-        mbar_wait(&ctl.tmem_full[as], aphase, 10);
-        tc_fence_after();
-        const long long m = (long long)tm * 128 + warp * 32 + lane;
+      } else {
+        // 32-column slices through one smem tile: thread t then holds row t of the slice
+        const long long m = (long long)tm * 128 + threadIdx.x;
         long long row_off = m * g.ldc;
         if (g.os && m < g.M) {       // scattered rows (strided-dgrad parity class)
           uint32_t n, rem, p, q;
@@ -344,62 +296,49 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
           g.dQ.divmod(rem, p, q);
           row_off = (((long long)n * g.OH + p * g.os + g.oh0) * g.OW + q * g.os + g.ow0) * g.ldc;
         }
-        const uint32_t tbase = tmem_base + (uint32_t)(as * BN) + ((uint32_t)(warp * 32) << 16);
-#pragma unroll 1
+#pragma unroll
         for (int c = 0; c < BN / 32; ++c) {
-          uint32_t acc[32];
-          tmem_ld32(tbase + c * 32, acc);
-          tmem_ld_wait();
           const int n0 = tn * BN + c * 32;
           const int valid = g.n_out - n0;
-          if (m < g.M && valid > 0) {
+          if (valid <= 0) continue;                        // uniform across the CTA
+          named_barrier_sync(1, EPI_THREADS);              // the previous slice has been read
+          stage_frag<float>(smem_u32(ctl.epi), acc, c * 4, all_rows);
+          named_barrier_sync(1, EPI_THREADS);
+          uint32_t r32[32];
+          load_row32(ctl.epi, threadIdx.x, r32);
+          if (m < g.M) {
             if (sizeof(To) == 4 && g.accum) {
               float* o = reinterpret_cast<float*>(out) + row_off + n0;
 #pragma unroll
-              for (int i = 0; i < 32; ++i) if (i < valid) atomicAdd(o + i, __uint_as_float(acc[i]));
+              for (int i = 0; i < 32; ++i) if (i < valid) atomicAdd(o + i, __uint_as_float(r32[i]));
             } else {
-              store_row32<To>(out + row_off + n0, acc, valid, vec_ok);
+              store_row32<To>(out + row_off + n0, r32, valid, vec_ok);
             }
           }
         }
-        tc_fence_before();
-        warp_arrive(&ctl.tmem_empty[as]);
-        as ^= 1; if (as == 0) aphase ^= 1;
       }
     }
-  } else if (warp == 4) {
-    // ------------------------------ MMA issuer ----------------------------
-    // All lanes run the loop on warp-uniform values; the descriptor low words are running 32-bit sums (one
-    // uniform add per MMA) and one elected lane issues the four MMAs of a stage back to back.  Building each
-    // 64-bit descriptor from an address inside `if (lane == 0)` cost ~20 SASS instructions per MMA and paced
-    // short-N tiles at ~130 cycles per MMA instead of 32-128 (profiles/r02_ncu_halo.txt).
-    constexpr uint32_t HI = desc_hi_sw128(1024);
-    Pipe pp{0, 0};
-    int as = 0; uint32_t aphase = 0;
-    const uint32_t smem_lo = uniform_u32(desc_lo(smem_u32(smem), 16));
-    const uint32_t tmem_u = uniform_u32(tmem_base);
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      mbar_wait(&ctl.tmem_empty[as], aphase ^ 1, 20);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_u + (uint32_t)(as * BN);
-      for (int kb = 0; kb < g.num_kb; ++kb) {
-        mbar_wait(&ctl.full[pp.stage], pp.phase, 21);
-        tc_fence_after();
-        const uint32_t a_lo = smem_lo + (uint32_t)pp.stage * (TL::STAGE_BYTES >> 4);
-        const uint32_t b_lo = a_lo + (A_STAGE_BYTES >> 4);
-        if (elect_one()) {
+    if (TMA_EPI && STATS && !STATS_WARPS) {
+      const int tn0 = blockIdx.x % g.tiles_n;            // constant for this CTA (gridDim % tiles_n == 0)
 #pragma unroll
-          for (int k = 0; k < 4; ++k)        // 4 x (32 bytes of K) per stage
-            umma<TF32>(d_tmem, desc_pack(a_lo + 2 * k, HI), desc_pack(b_lo + 2 * k, HI), IDESC, (kb | k) != 0 ? 1u : 0u);
-          umma_commit(&ctl.empty[pp.stage]);            // frees the smem slot when the MMAs retire
-          if (kb == g.num_kb - 1) umma_commit(&ctl.tmem_full[as]);
+      for (int b = 0; b < BOXES; ++b) {
+#pragma unroll
+        for (int c = 0; c < CPC; ++c) {
+          // fold the 4 row groups of the warp (lane >> 3) onto lanes 0-7
+          float s0 = st_sum[b][c], s1 = st_sq[b][c];
+          s0 += __shfl_xor_sync(0xffffffffu, s0, 8);  s1 += __shfl_xor_sync(0xffffffffu, s1, 8);
+          s0 += __shfl_xor_sync(0xffffffffu, s0, 16); s1 += __shfl_xor_sync(0xffffffffu, s1, 16);
+          const int col = tn0 * BN + b * BOX_COLS + sj * CPC + c;
+          if (lane < 8 && col < g.n_out && (int)blockIdx.x < num_tiles) {     // partial of (CTA, warp): summed in order
+            double* part = bn_sums + ((size_t)blockIdx.x * 4 + warp) * 2 * g.n_out;
+            part[col] = (double)s0;
+            part[g.n_out + col] = (double)s1;
+          }
         }
-        __syncwarp();
-        advance<STAGES>(pp);
       }
-      as ^= 1; if (as == 0) aphase ^= 1;
     }
-  } else if (warp == 5) {
+    if (TMA_EPI && threadIdx.x == 0) tma_store_wait_all<0>();
+  } else if (warp == 4) {
     // ------------------------------ TMA producer --------------------------
     if (lane == 0) {
       Pipe pp{0, 0};
@@ -414,7 +353,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
           im_n = (int)n; im_w = (int)q * g.stride + g.im_base; im_h = (int)p * g.stride + g.im_base;
         }
         for (int kb = 0; kb < g.num_kb; ++kb) {
-          mbar_wait(&ctl.empty[pp.stage], pp.phase ^ 1, 30);
+          mbar_wait(&ctl.empty[pp.stage], pp.phase ^ 1);
           uint8_t* a_dst = smem + (size_t)pp.stage * TL::STAGE_BYTES;
           mbar_arrive_expect_tx(&ctl.full[pp.stage], TL::B_STAGE_BYTES + (A_TMA ? A_STAGE_BYTES : 0));
           if (A_TMA) {
@@ -440,7 +379,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
   } else {
     // ------------------------------ statistics warps (TMA-fed kernels) -----
     if (STATS_WARPS) {
-      const int st_t = threadIdx.x - 192;
+      const int st_t = threadIdx.x - AUX_T0;
       const int sj = st_t & 7, srg = st_t >> 3;
       // packed fp32 pairs: (sum, sum) and (sumsq, sumsq) of two adjacent columns per register pair
       constexpr int CP2 = CPC / 2;
@@ -456,7 +395,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
         for (int b = 0; b < BOXES; ++b) {
           if (tn * BN + b * BOX_COLS >= g.n_out) continue;
           const uint8_t* stage = ctl.epi + (ctr & 1) * A_STAGE_BYTES;
-          mbar_wait(&ctl.sfull[ctr & 1], (ctr >> 1) & 1, 45);
+          mbar_wait(&ctl.sfull[ctr & 1], (ctr >> 1) & 1);
 #pragma unroll
           for (int i = 0; i < 8; ++i) {                     // rows srg*8 + i (rows >= M hold exact zeros)
             const uint4 raw = *reinterpret_cast<const uint4*>(stage + (srg * 8 + i) * 128 + ((sj ^ i) << 4));
@@ -480,9 +419,8 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
         }
       }
       // Flush: fold the row groups of a warp by shuffles, the four warps through shared memory (the
-      // operand ring is idle by now: every MMA of this CTA has retired), then ONE fp64 atomic per
-      // column per CTA -- same-address atomics serialise in L2 (~30 ns each), so their count per
-      // column, not their total, sets the tail of the kernel.
+      // operand ring is idle by now: every MMA of this CTA has retired before its last box was staged), then ONE fp64 partial
+      // per column per CTA into the CTA's slot of the partials, which the host adds in CTA order.
       const int tn0 = blockIdx.x % g.tiles_n;
       float* red = reinterpret_cast<float*>(smem);          // [4 warps][BN columns][2]
       const int sw = st_t >> 5;
@@ -506,8 +444,9 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
           double s0 = 0.0, s1 = 0.0;
 #pragma unroll
           for (int w = 0; w < 4; ++w) { s0 += (double)red[(w * BN + lc) * 2]; s1 += (double)red[(w * BN + lc) * 2 + 1]; }
-          atomicAdd(bn_sums + col, s0);
-          atomicAdd(bn_sums + g.n_out + col, s1);
+          double* part = bn_sums + (size_t)blockIdx.x * 4 * 2 * g.n_out;
+          part[col] = s0;
+          part[g.n_out + col] = s1;
         }
       }
     }
@@ -516,7 +455,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
     // MMA warp (fence.proxy.async + mbarrier arrive) once its group has landed.
     if (!A_TMA) {
       constexpr int D = TL::GATHER_DEPTH;
-      const int gt = threadIdx.x - 192;
+      const int gt = threadIdx.x - AUX_T0;
       const int j = gt & 7;              // 16-byte chunk within the 128-byte K block
       const int row0 = gt >> 3;          // rows row0 + GROWS*i
       Pipe pi{0, 0}, pa{0, 0};
@@ -539,7 +478,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
         const T* src = reinterpret_cast<const T*>(g.src);
         for (int kb = 0; kb < g.num_kb; ++kb) {
           const uint32_t k0 = (uint32_t)(kb * KBE + j * CH);
-          mbar_wait(&ctl.empty[pi.stage], pi.phase ^ 1, 40);
+          mbar_wait(&ctl.empty[pi.stage], pi.phase ^ 1);
           const uint32_t a_addr = smem_u32(smem + (size_t)pi.stage * TL::STAGE_BYTES);
           if (!SMALLC) {
             uint32_t tap, c; g.dC.divmod(k0, tap, c);
@@ -583,34 +522,32 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
     }
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (warp == 4) { tc_fence_after(); tmem_dealloc(tmem_base, TL::TMEM_COLS); }
 }
 
 // ===========================================================================
 // wgrad:  dW[(r,s,c)][co] = sum_pixels X[pixel@(r,s)][c] * dY[pixel][co]
 // A^T (activations) and B (dY) are both MN-major: the reduction runs over pixels.
-// Work item = (128 k-rows) x (BN couts) x (pixel split); fp32 atomics combine splits.
+// Work item = (128 k-rows) x (BN couts) x (pixel split).  With one split every dW element is written once; with
+// several, each split writes its partial to scratch and run_sum_partials adds them in split order (deterministic).
 // ===========================================================================
-template <typename T, int BN, bool SMALLC, bool A_TMA, bool TMA_RED, int MT = 1>
+template <typename T, int BN, bool SMALLC, bool A_TMA, bool TMA_RED>
 __global__ void __launch_bounds__(wgrad_threads(A_TMA), 1)
 wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_dy,
              const __grid_constant__ CUtensorMap tmap_dw, const Geom g, float* __restrict__ dw) {
-  using TL = WTile<BN, MT>;
+  using TL = WTile<BN>;
   constexpr int STAGES = TL::STAGES;
-  constexpr int NACC = TL::NACC;
-  static_assert(MT == 1 || (A_TMA && TMA_RED && !SMALLC), "256-row tiles: TMA-fed, reduce-add epilogue only");
-  constexpr bool TF32 = Elt<T>::TF32;
+  static_assert(!Elt<T>::TF32, "MN-major fp32 operands: not supported by wgmma");
   constexpr int ATOM_E = Elt<T>::KBE;            // elements along MN per 128-byte atom row
   constexpr int CH = Elt<T>::CH;
-  constexpr int A_ATOMS = 128 / ATOM_E;          // 2 (bf16) / 4 (fp32)
-  constexpr int PXS = A_STAGE_BYTES / (A_ATOMS * 128);   // pixels per stage: 64 / 32
-  constexpr int UMMA_K = 32 / (int)sizeof(T);    // 16 / 8 pixels per MMA
+  constexpr int A_ATOMS = 128 / ATOM_E;          // 2
+  constexpr int PXS = A_STAGE_BYTES / (A_ATOMS * 128);   // pixels per stage: 64
+  constexpr int MMA_K = 32 / (int)sizeof(T);    // 16 pixels per MMA
   constexpr int ATOM_BYTES = PXS * 128;
   constexpr int B_ATOMS = BN / ATOM_E;
-  constexpr uint32_t IDESC = make_idesc(TF32, 128, BN, true, true);
-  static_assert(PXS / UMMA_K == 4, "4 MMAs per stage");
+  constexpr int NF = BN / 2;
+  static_assert(PXS / MMA_K == 4, "4 MMAs per stage");
+  static_assert(A_ATOMS == 2, "one 64-row atom per m64 half");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -618,20 +555,15 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&ctl.full[s], A_TMA ? 1 : 1 + GATHER_THREADS / 32); mbar_init(&ctl.empty[s], 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&ctl.tmem_full[a], 1); mbar_init(&ctl.tmem_empty[a], EPI_THREADS / 32); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&ctl.full[s], A_TMA ? 1 : 1 + GATHER_THREADS / 32); mbar_init(&ctl.empty[s], EPI_THREADS / 32); }
     fence_barrier_init();
   }
-  if (warp == 5 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     tma_prefetch_desc(&tmap_dy);
     if (A_TMA) tma_prefetch_desc(&tmap_x);
     if (TMA_RED) tma_prefetch_desc(&tmap_dw);
   }
-  if (warp == 4) tmem_alloc(ctl.tmem_ptr, TL::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *ctl.tmem_ptr;
   const int num_items = g.tiles_m * g.tiles_n * g.splits;   // tiles_m = k-row tiles
 
   // item -> (tk, tn, split); splits of one tile are adjacent so their dY reads share L2
@@ -644,43 +576,60 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
   };
 
   if (warp < 4) {
-    int as = 0; uint32_t aphase = 0;
+    // ------------------------------ consumer: MMA + epilogue ------------------------------
+    // MN-major operands: LBO = distance between 128-byte-wide atoms along M/N, SBO = 8 pixel rows; the m64 half h
+    // of the A tile is atom h
+    constexpr uint32_t HI = desc_hi_sw128(1024);
+    const uint32_t smem_lo = uniform_u32(desc_lo(smem_u32(smem), ATOM_BYTES));
+    const bool all_rows[2][2] = {{true, true}, {true, true}};
+    float acc[2][NF];
+    Pipe pp{0, 0};
     uint32_t box_ctr = 0;
     for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
       int tk, tn, kb0, kb1; decode(item, tk, tn, kb0, kb1);
       if (kb0 >= kb1) continue;
-      mbar_wait(&ctl.tmem_full[as], aphase, 50);
-      tc_fence_after();
-      const uint32_t tbase = tmem_base + (uint32_t)(as * MT * BN) + ((uint32_t)(warp * 32) << 16);
+      const int split = item % g.splits;
+      int prev = 0;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&ctl.full[pp.stage], pp.phase);
+        const uint32_t a_lo = smem_lo + (uint32_t)pp.stage * (TL::STAGE_BYTES >> 4);
+        const uint32_t b_lo = a_lo + (TL::A_BYTES >> 4);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            wgmma<BN, false, true, true>(acc[h], desc_pack(a_lo + h * (ATOM_BYTES >> 4) + k * (MMA_K * 128 >> 4), HI),
+                                         desc_pack(b_lo + k * (MMA_K * 128 >> 4), HI), (kb > kb0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        if (kb > kb0) { wgmma_wait<1>(); warp_arrive(&ctl.empty[prev]); }
+        prev = pp.stage;
+        advance<STAGES>(pp);
+      }
+      wgmma_wait<0>(acc);
+      warp_arrive(&ctl.empty[prev]);
       if (TMA_RED) {
-        // partial tile -> swizzled smem [128 k-rows][32 fp32] -> TMA reduce-add into dW (splits combine at L2)
-        const int row = warp * 32 + lane;
-#pragma unroll 1
-        for (int cm = 0; cm < MT * (BN / 32); ++cm, ++box_ctr) {
-          const int mt = cm / (BN / 32), cc = cm - mt * (BN / 32);
+        // partial tile -> swizzled smem [128 k-rows][32 fp32] -> TMA reduce-add into dW, or TMA store into this
+        // split's rows of the scratch partials
+#pragma unroll
+        for (int cc = 0; cc < BN / 32; ++cc) {
           uint8_t* stage = ctl.epi + (box_ctr & 1) * A_STAGE_BYTES;
           const int n0 = tn * BN + cc * 32;
-          const bool live = n0 < g.Cout;
-          if (live) {
-            if (threadIdx.x == 0) tma_store_wait_read<1>();
-            named_barrier_sync(1, EPI_THREADS);
+          if (n0 >= g.Cout) continue;                      // uniform across the CTA
+          if (threadIdx.x == 0) tma_store_wait_read<1>();
+          named_barrier_sync(1, EPI_THREADS);
+          stage_frag<float>(smem_u32(stage), acc, cc * 4, all_rows);
+          fence_proxy_async();
+          named_barrier_sync(1, EPI_THREADS);
+          if (threadIdx.x == 0) {
+            if (g.ws) tma_store_2d(&tmap_dw, stage, n0, split * g.tiles_m * 128 + tk * 128);
+            else tma_reduce_add_2d(&tmap_dw, stage, n0, tk * 128);
+            tma_store_commit();
           }
-          uint32_t acc[32];
-          tmem_ld32(tbase + mt * BN + cc * 32, acc);
-          tmem_ld_wait();
-          if (cm == MT * (BN / 32) - 1) { tc_fence_before(); warp_arrive(&ctl.tmem_empty[as]); }
-          if (live) {
-            const uint32_t srow = smem_u32(stage);
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-              sts16(srow + sw128_offset(row, q), make_uint4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]));
-            fence_proxy_async();
-            named_barrier_sync(1, EPI_THREADS);
-            if (threadIdx.x == 0) { tma_reduce_add_2d(&tmap_dw, stage, n0, (tk * MT + mt) * 128); tma_store_commit(); }
-          }
+          ++box_ctr;
         }
       } else {
-        const int k = tk * 128 + warp * 32 + lane;           // row of the [R*S*Cs][Cout] matrix
+        const int k = tk * 128 + threadIdx.x;              // row of the [R*S*Cs][Cout] matrix
         uint32_t tap, c; bool row_ok;
         if (g.s2) {          // stem K order: (r, s' in [0, S], c in [0, 4)); s' = 0 is the zero slot
           const int t4 = k >> 2, r = t4 / g.s2, sp = t4 - r * g.s2;
@@ -691,66 +640,35 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
           g.dC.divmod((uint32_t)k, tap, c);
           row_ok = (int)tap < g.RS && (int)c < g.Cin;
         }
-        float* drow = dw + ((long long)tap * g.Cin + c) * g.Cout;
-#pragma unroll 1
+        // dW layout either way; several splits write their own copy of it
+        float* drow = (g.ws ? g.ws + split * g.ws_stride : dw) + ((long long)tap * g.Cin + c) * g.Cout;
+#pragma unroll
         for (int cc = 0; cc < BN / 32; ++cc) {
-          uint32_t acc[32];
-          tmem_ld32(tbase + cc * 32, acc);
-          tmem_ld_wait();
+          named_barrier_sync(1, EPI_THREADS);              // the previous slice has been read
+          stage_frag<float>(smem_u32(ctl.epi), acc, cc * 4, all_rows);
+          named_barrier_sync(1, EPI_THREADS);
+          uint32_t r32[32];
+          load_row32(ctl.epi, threadIdx.x, r32);
           const int n0 = tn * BN + cc * 32;
           if (row_ok) {
 #pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (n0 + i < g.Cout) atomicAdd(drow + n0 + i, __uint_as_float(acc[i]));
+            for (int i = 0; i < 32; ++i) {
+              if (n0 + i >= g.Cout) continue;
+              if (g.ws) drow[n0 + i] = __uint_as_float(r32[i]);
+              else atomicAdd(drow + n0 + i, __uint_as_float(r32[i]));     // the only write to this element
+            }
           }
         }
-        tc_fence_before();
-        warp_arrive(&ctl.tmem_empty[as]);
       }
-      if (++as == NACC) { as = 0; aphase ^= 1; }
     }
     if (TMA_RED && threadIdx.x == 0) tma_store_wait_all<0>();
   } else if (warp == 4) {
-    // MN-major operands: LBO = distance between 128-byte-wide atoms along M/N, SBO = 8 pixel rows; uniform
-    // running descriptor words, one elected lane issues the four MMAs of a stage (see igemm_kernel)
-    constexpr uint32_t HI = desc_hi_sw128(1024);
-    Pipe pp{0, 0};
-    int as = 0; uint32_t aphase = 0;
-    const uint32_t smem_lo = uniform_u32(desc_lo(smem_u32(smem), ATOM_BYTES));
-    const uint32_t tmem_u = uniform_u32(tmem_base);
-    for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-      int tk, tn, kb0, kb1; decode(item, tk, tn, kb0, kb1);
-      if (kb0 >= kb1) continue;
-      mbar_wait(&ctl.tmem_empty[as], aphase ^ 1, 60);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_u + (uint32_t)(as * MT * BN);
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&ctl.full[pp.stage], pp.phase, 61);
-        tc_fence_after();
-        const uint32_t a_lo = smem_lo + (uint32_t)pp.stage * (TL::STAGE_BYTES >> 4);
-        const uint32_t b_lo = a_lo + (TL::A_BYTES >> 4);
-        if (elect_one()) {
-#pragma unroll
-          for (int mt = 0; mt < MT; ++mt)
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma<TF32>(d_tmem + mt * BN, desc_pack(a_lo + mt * (A_STAGE_BYTES >> 4) + k * (UMMA_K * 128 >> 4), HI),
-                         desc_pack(b_lo + k * (UMMA_K * 128 >> 4), HI), IDESC, (kb > kb0 || k > 0) ? 1u : 0u);
-          umma_commit(&ctl.empty[pp.stage]);
-          if (kb == kb1 - 1) umma_commit(&ctl.tmem_full[as]);
-        }
-        __syncwarp();
-        advance<STAGES>(pp);
-      }
-      if (++as == NACC) { as = 0; aphase ^= 1; }
-    }
-  } else if (warp == 5) {
     if (lane == 0) {
       Pipe pp{0, 0};
       for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
         int tk, tn, kb0, kb1; decode(item, tk, tn, kb0, kb1);
         for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&ctl.empty[pp.stage], pp.phase ^ 1, 70);
+          mbar_wait(&ctl.empty[pp.stage], pp.phase ^ 1);
           uint8_t* a_dst = smem + (size_t)pp.stage * TL::STAGE_BYTES;
           uint8_t* b_dst = a_dst + TL::A_BYTES;
           mbar_arrive_expect_tx(&ctl.full[pp.stage], TL::B_STAGE_BYTES + (A_TMA ? TL::A_BYTES : 0));
@@ -760,9 +678,9 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
               g.dPQ.divmod((uint32_t)(kb * PXS), n, rem);
               g.dQ.divmod(rem, p, q);
 #pragma unroll
-              for (int a = 0; a < MT * A_ATOMS; ++a) {
+              for (int a = 0; a < A_ATOMS; ++a) {
                 uint32_t tap, c, r, s2;
-                g.dC.divmod((uint32_t)(tk * MT * 128 + a * ATOM_E), tap, c);
+                g.dC.divmod((uint32_t)(tk * 128 + a * ATOM_E), tap, c);
                 g.dS.divmod(tap, r, s2);
                 const bool live = (int)tap < g.RS;     // k-rows past R*S*C: read a non-existent image (zeros)
                 tma_load_im2col(a_dst + a * ATOM_BYTES, &tmap_x, &ctl.full[pp.stage], (int)c,
@@ -771,8 +689,8 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
               }
             } else {         // 1x1 stride-1: the activation tile is a plain [pixels][channels] box
 #pragma unroll
-              for (int a = 0; a < MT * A_ATOMS; ++a)
-                tma_load_2d(a_dst + a * ATOM_BYTES, &tmap_x, &ctl.full[pp.stage], tk * MT * 128 + a * ATOM_E, kb * PXS);
+              for (int a = 0; a < A_ATOMS; ++a)
+                tma_load_2d(a_dst + a * ATOM_BYTES, &tmap_x, &ctl.full[pp.stage], tk * 128 + a * ATOM_E, kb * PXS);
             }
           }
 #pragma unroll
@@ -785,7 +703,7 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
     __syncwarp();
   } else if (!A_TMA) {
     constexpr int D = TL::GATHER_DEPTH;
-    const int gt = threadIdx.x - 192;
+    const int gt = threadIdx.x - AUX_T0;
     const int j = gt & 7;
     Pipe pi{0, 0}, pa{0, 0};
     int inflight = 0;
@@ -826,7 +744,7 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
         sn[e] = (int)nn; sp[e] = (int)p; sq[e] = (int)qq;
       }
       for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&ctl.empty[pi.stage], pi.phase ^ 1, 80);
+        mbar_wait(&ctl.empty[pi.stage], pi.phase ^ 1);
         const uint32_t a_addr = smem_u32(smem + (size_t)pi.stage * TL::STAGE_BYTES);
 #pragma unroll
         for (int i = 0; i < GPT; ++i) {
@@ -875,15 +793,13 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
     for (; inflight > 0; --inflight) { warp_arrive(&ctl.full[pa.stage]); advance<STAGES>(pa); }
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (warp == 4) { tc_fence_after(); tmem_dealloc(tmem_base, TL::TMEM_COLS); }
 }
 
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
-inline int pick_bn(int64_t n) { return n > 128 ? 256 : (n > 64 ? 128 : 64); }
+inline int pick_bn(int64_t n) { return n > 64 ? 128 : 64; }
 
 template <typename K> int set_smem_attr(K kernel, size_t bytes) {
   cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
@@ -891,16 +807,23 @@ template <typename K> int set_smem_attr(K kernel, size_t bytes) {
   return SIMCLR_OK;
 }
 
+// CTAs of an igemm launch.  With fused statistics each CTA keeps one column block (tile = blockIdx.x + i*gridDim.x
+// keeps tn fixed), so the grid is a multiple of tiles_n.
+inline int igemm_grid(const Geom& g, bool stats) {
+  int grid = g.tiles_m * g.tiles_n; if (grid > num_sms()) grid = num_sms();
+  if (stats) {
+    grid = grid / g.tiles_n * g.tiles_n;
+    if (grid < g.tiles_n) grid = g.tiles_n;
+  }
+  return grid;
+}
+
 template <typename T, typename To, int BN, bool A_TMA, bool SMALLC, bool TMA_EPI, bool STATS>
 int launch_igemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout, const Geom& g, double* bn_sums,
                  cudaStream_t st) {
   auto kern = igemm_kernel<T, To, BN, A_TMA, SMALLC, TMA_EPI, STATS>;
   { int rc = set_smem_attr(kern, Tile<BN>::SMEM_BYTES); if (rc) return rc; }   // a per-DEVICE attribute: set on every launch
-  int grid = g.tiles_m * g.tiles_n; if (grid > num_sms()) grid = num_sms();
-  if (STATS) {                 // one column block per CTA: tile = blockIdx.x + i*gridDim.x keeps tn fixed
-    grid = grid / g.tiles_n * g.tiles_n;
-    if (grid < g.tiles_n) grid = g.tiles_n;
-  }
+  const int grid = igemm_grid(g, STATS);
   kern<<<grid, igemm_threads(A_TMA, STATS), Tile<BN>::SMEM_BYTES, st>>>(ta, tb, tout, g, bn_sums);
   SIMCLR_CHECK_LAUNCH();
   return SIMCLR_OK;
@@ -923,7 +846,6 @@ int dispatch_igemm2(bool a_tma, bool smallc, bool tma_epi, const CUtensorMap& ta
 template <typename T, typename To>
 int dispatch_igemm(int bn, bool a_tma, bool smallc, bool tma_epi, const CUtensorMap& ta, const CUtensorMap& tb,
                    const CUtensorMap& tout, const Geom& g, cudaStream_t st, double* bn_sums = nullptr) {
-  if (bn == 256) return dispatch_igemm2<T, To, 256>(a_tma, smallc, tma_epi, ta, tb, tout, g, bn_sums, st);
   if (bn == 128) return dispatch_igemm2<T, To, 128>(a_tma, smallc, tma_epi, ta, tb, tout, g, bn_sums, st);
   return dispatch_igemm2<T, To, 64>(a_tma, smallc, tma_epi, ta, tb, tout, g, bn_sums, st);
 }
@@ -1041,12 +963,28 @@ int run_igemm(int mode, const void* src, const void* wk, void* out, int dtype, i
   const bool tma_epi = aligned16(out) && ((n_out * eo) % 16 == 0);
   if (tma_epi) { rc = make_tmap_2d(&tout, out, eo, (uint64_t)M, (uint64_t)n_out, (uint64_t)n_out * eo, 128, (uint32_t)(128 / eo)); if (rc) return rc; }
   else tout = tb;
+  double* parts = nullptr;            // fused statistics: [CTAs][4 warps][2][n_out] partials, added in order
+  const int nparts = 4 * igemm_grid(g, true);
   if (bn_sums) {
     if (!tma_epi) { set_error("%s: fused BN statistics need 16-byte aligned output rows", what); return SIMCLR_ERR_UNSUPPORTED; }
     if (!accumulate_prezeroed()) {
       cudaError_t e = cudaMemsetAsync(bn_sums, 0, 2 * (size_t)n_out * sizeof(double), st);
       if (e != cudaSuccess) { set_error("%s: memset: %s", what, cudaGetErrorString(e)); return (int)e; }
     }
+    rc = scratch_alloc(&parts, (size_t)nparts * 2 * n_out * sizeof(double), st);
+    if (rc) return rc;
+    cudaError_t e = cudaMemsetAsync(parts, 0, (size_t)nparts * 2 * n_out * sizeof(double), st);
+    if (e != cudaSuccess) { set_error("%s: memset: %s", what, cudaGetErrorString(e)); scratch_free(parts, st); return (int)e; }
+    if (dtype == SIMCLR_BF16 && out_dtype == SIMCLR_BF16)
+      rc = dispatch_igemm<__nv_bfloat16, __nv_bfloat16>(bn, a_tma, smallc, tma_epi, ta, tb, tout, g, st, parts);
+    else if (dtype == SIMCLR_BF16 && out_dtype == SIMCLR_F32)
+      rc = dispatch_igemm<__nv_bfloat16, float>(bn, a_tma, smallc, tma_epi, ta, tb, tout, g, st, parts);
+    else if (dtype == SIMCLR_F32 && out_dtype == SIMCLR_F32)
+      rc = dispatch_igemm<float, float>(bn, a_tma, smallc, tma_epi, ta, tb, tout, g, st, parts);
+    else { set_error("%s: unsupported dtype combination %d -> %d", what, dtype, out_dtype); rc = SIMCLR_ERR_UNSUPPORTED; }
+    if (!rc) rc = run_sum_partials_f64(parts, 2 * n_out, bn_sums, 2 * n_out, nparts, st);
+    const int rf = scratch_free(parts, st);
+    return rc ? rc : rf;
   }
   if (dtype == SIMCLR_BF16 && out_dtype == SIMCLR_BF16) return dispatch_igemm<__nv_bfloat16, __nv_bfloat16>(bn, a_tma, smallc, tma_epi, ta, tb, tout, g, st, bn_sums);
   if (dtype == SIMCLR_BF16 && out_dtype == SIMCLR_F32) return dispatch_igemm<__nv_bfloat16, float>(bn, a_tma, smallc, tma_epi, ta, tb, tout, g, st, bn_sums);
@@ -1142,13 +1080,13 @@ int run_dgrad_strided(const void* dy, const void* wd, void* dx, int dtype, int o
   return SIMCLR_OK;
 }
 
-template <typename T, int BN, bool SMALLC, bool A_TMA, bool TMA_RED, int MT = 1>
+template <typename T, int BN, bool SMALLC, bool A_TMA, bool TMA_RED>
 int launch_wgrad(const CUtensorMap& tx, const CUtensorMap& tdy, const CUtensorMap& tdw, const Geom& g, float* dw,
                  cudaStream_t st) {
-  auto kern = wgrad_kernel<T, BN, SMALLC, A_TMA, TMA_RED, MT>;
-  int rc = set_smem_attr(kern, WTile<BN, MT>::SMEM_BYTES); if (rc) return rc;      // per device: set every time
+  auto kern = wgrad_kernel<T, BN, SMALLC, A_TMA, TMA_RED>;
+  int rc = set_smem_attr(kern, WTile<BN>::SMEM_BYTES); if (rc) return rc;      // per device: set every time
   int grid = g.tiles_m * g.tiles_n * g.splits; if (grid > num_sms()) grid = num_sms();
-  kern<<<grid, wgrad_threads(A_TMA), WTile<BN, MT>::SMEM_BYTES, st>>>(tx, tdy, tdw, g, dw);
+  kern<<<grid, wgrad_threads(A_TMA), WTile<BN>::SMEM_BYTES, st>>>(tx, tdy, tdw, g, dw);
   SIMCLR_CHECK_LAUNCH();
   return SIMCLR_OK;
 }
@@ -1157,7 +1095,6 @@ int dispatch_wgrad2(bool smallc, bool a_tma, bool tma_red, const CUtensorMap& tx
                     const CUtensorMap& tdw, const Geom& g, float* dw, cudaStream_t st) {
   if (smallc) return launch_wgrad<T, BN, true, false, false>(tx, tdy, tdw, g, dw, st);
   if (tma_red) {
-    if (a_tma && g.wg_mt == 2) return launch_wgrad<T, BN, false, true, true, 2>(tx, tdy, tdw, g, dw, st);
     if (a_tma) return launch_wgrad<T, BN, false, true, true>(tx, tdy, tdw, g, dw, st);
     return launch_wgrad<T, BN, false, false, true>(tx, tdy, tdw, g, dw, st);
   }
@@ -1167,13 +1104,56 @@ int dispatch_wgrad2(bool smallc, bool a_tma, bool tma_red, const CUtensorMap& tx
 template <typename T>
 int dispatch_wgrad(int bn, bool smallc, bool a_tma, bool tma_red, const CUtensorMap& tx, const CUtensorMap& tdy,
                    const CUtensorMap& tdw, const Geom& g, float* dw, cudaStream_t st) {
-  if (bn == 256) return dispatch_wgrad2<T, 256>(smallc, a_tma, tma_red, tx, tdy, tdw, g, dw, st);
   if (bn == 128) return dispatch_wgrad2<T, 128>(smallc, a_tma, tma_red, tx, tdy, tdw, g, dw, st);
   return dispatch_wgrad2<T, 64>(smallc, a_tma, tma_red, tx, tdy, tdw, g, dw, st);
 }
 
 }  // namespace
+
 }  // namespace tc
+
+// A block takes 32 consecutive elements; lane ty of 16 adds parts ty, ty + 16, ... in order, then the 16 lane sums are
+// added in lane order.  The order depends only on `parts`, so the result is the same on every run.
+constexpr int SUM_LANES = 16;
+template <typename T>
+__global__ void __launch_bounds__(32 * SUM_LANES) sum_partials_kernel(const T* __restrict__ ws, long long stride, T* __restrict__ dst,
+                                                                      long long n, int parts) {
+  __shared__ T sh[SUM_LANES][33];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  for (long long i0 = blockIdx.x * 32ll; i0 < n; i0 += (long long)gridDim.x * 32) {
+    const long long i = i0 + tx;
+    T a = 0;
+    if (i < n)
+      for (int p = ty; p < parts; p += SUM_LANES) a += ws[p * stride + i];
+    sh[ty][tx] = a;
+    __syncthreads();
+    if (ty == 0 && i < n) {
+      T d = dst[i];
+#pragma unroll
+      for (int k = 0; k < SUM_LANES; ++k) d += sh[k][tx];
+      dst[i] = d;
+    }
+    __syncthreads();
+  }
+}
+
+template <typename T>
+int sum_partials(const T* ws, int64_t stride, T* dst, int64_t n, int parts, cudaStream_t st) {
+  int64_t blocks = (n + 31) / 32;
+  if (blocks > 16 * (int64_t)num_sms()) blocks = 16 * (int64_t)num_sms();
+  if (blocks < 1) blocks = 1;
+  sum_partials_kernel<T><<<(int)blocks, 32 * SUM_LANES, 0, st>>>(ws, stride, dst, n, parts);
+  SIMCLR_CHECK_LAUNCH();
+  return SIMCLR_OK;
+}
+
+int run_sum_partials(const float* ws, int64_t stride, float* dst, int64_t n, int parts, cudaStream_t st) {
+  return sum_partials(ws, stride, dst, n, parts, st);
+}
+int run_sum_partials_f64(const double* ws, int64_t stride, double* dst, int64_t n, int parts, cudaStream_t st) {
+  return sum_partials(ws, stride, dst, n, parts, st);
+}
+
 }  // namespace simclr
 
 using namespace simclr;
@@ -1221,8 +1201,7 @@ static int wgrad_tc_impl(const void* x, const void* dy, float* dw, int dtype, in
                    "conv2d_wgrad_tc: bad geometry");
   cudaStream_t st = (cudaStream_t)stream;
   if (dtype == SIMCLR_F32) {
-    // 32-bit MN-major operands need the 128B_BASE32B swizzle atom, which this kernel does not
-    // implement; fp32 storage is the verification mode and takes its wgrad from the CUDA-core engine.
+    // wgmma takes tf32 operands K-major only, and both wgrad operands are MN-major; fp32 storage is the verification mode and takes its wgrad from the CUDA-core engine.
     set_error("conv2d_wgrad_tc: fp32 operands are not supported (use conv2d_wgrad_simt)");
     return SIMCLR_ERR_UNSUPPORTED;
   }
@@ -1258,8 +1237,9 @@ static int wgrad_tc_impl(const void* x, const void* dy, float* dw, int dtype, in
   g.M = M; g.n_out = (int)Cout; g.ldc = (int)Cout;
   g.num_kb = (int)((M + pxs - 1) / pxs);
   g.tiles_m = (int)((R * Sk * Cs + 127) / 128); g.tiles_n = (int)((Cout + bn - 1) / bn);
-  g.Cin = (int)Cin; g.Cout = (int)Cout; g.wg_mt = 1;
+  g.Cin = (int)Cin; g.Cout = (int)Cout;
   g.use_tab = 0; g.cblocks = 1; g.os = 0; g.oh0 = g.ow0 = 0; g.OH = g.OW = 0; g.tap_sign = 1; g.accum = 0;
+  g.ws = nullptr; g.ws_stride = 0;
   const int tiles = g.tiles_m * g.tiles_n;
   int splits = (2 * num_sms() + tiles - 1) / tiles;
   const int max_splits = g.num_kb / 8 > 0 ? g.num_kb / 8 : 1;
@@ -1285,30 +1265,25 @@ static int wgrad_tc_impl(const void* x, const void* dy, float* dw, int dtype, in
   // splits are combined by TMA reduce-add when dW is a plain [R*S*Cin][Cout] fp32 matrix with 16-byte rows
   CUtensorMap tdw;
   const bool tma_red = !stem && Cs == Cin && aligned16(dw) && (Cout * 4) % 16 == 0;
-  // 256-row work items (two accumulators per dY tile) when the filter matrix has whole 256-row tiles or is tall
-  // enough for the padding of the last one not to matter; SIMCLR_TC_WGRAD_MT=1 restores 128-row items (A/B runs)
-  {
-    static int mt_en = -1;
-    if (mt_en < 0) { const char* e = getenv("SIMCLR_TC_WGRAD_MT"); mt_en = (e && e[0] == '1') ? 0 : 1; }
-    const int64_t krows = R * Sk * Cs;
-    if (mt_en && a_tma && tma_red && !smallc && krows >= 256 && (krows % 256 == 0 || krows >= 1024)) {
-      g.wg_mt = 2;
-      g.tiles_m = (int)((krows + 255) / 256);
-      const int tiles2 = g.tiles_m * g.tiles_n;
-      int sp = (2 * num_sms() + tiles2 - 1) / tiles2;
-      const int max_sp = g.num_kb / 8 > 0 ? g.num_kb / 8 : 1;
-      if (sp > max_sp) sp = max_sp;
-      if (sp < 1) sp = 1;
-      g.kb_per_split = (g.num_kb + sp - 1) / sp;
-      g.splits = (g.num_kb + g.kb_per_split - 1) / g.kb_per_split;
-    }
+  const int64_t dw_elems = R * S * Cin * Cout;
+  if (dtype != SIMCLR_BF16) { set_error("conv2d_wgrad_tc: unknown dtype %d", dtype); return SIMCLR_ERR_INVALID_ARG; }
+  if (zero && !accumulate_prezeroed()) SIMCLR_CHECK_CUDA(cudaMemsetAsync(dw, 0, (size_t)dw_elems * sizeof(float), st));
+  if (g.splits == 1) {          // every dW element is written once: reduce-add / atomics straight into dW
+    if (tma_red) { rc = make_tmap_2d(&tdw, dw, 4, (uint64_t)(R * S * Cin), (uint64_t)Cout, (uint64_t)Cout * 4, 128, 32); if (rc) return rc; }
+    else tdw = tdy;
+    return dispatch_wgrad<__nv_bfloat16>(bn, smallc, a_tma, tma_red, tx, tdy, tdw, g, dw, st);
   }
-  if (tma_red) { rc = make_tmap_2d(&tdw, dw, 4, (uint64_t)(R * S * Cin), (uint64_t)Cout, (uint64_t)Cout * 4, 128, 32); if (rc) return rc; }
+  // partials: TMA-stored tiles [splits][tiles_m * 128 rows][Cout] (the rows of a split past R*S*Cin are never read),
+  // or the dW layout per split for the scattered (stem / padded-channel) rows
+  g.ws_stride = tma_red ? (long long)g.tiles_m * 128 * Cout : (long long)dw_elems;
+  rc = scratch_alloc(&g.ws, (size_t)g.splits * g.ws_stride * sizeof(float), st);
+  if (rc) return rc;
+  if (tma_red) rc = make_tmap_2d(&tdw, g.ws, 4, (uint64_t)g.splits * g.tiles_m * 128, (uint64_t)Cout, (uint64_t)Cout * 4, 128, 32);
   else tdw = tdy;
-  if (zero && !accumulate_prezeroed()) SIMCLR_CHECK_CUDA(cudaMemsetAsync(dw, 0, (size_t)(R * S * Cin * Cout) * sizeof(float), st));
-  if (dtype == SIMCLR_BF16) return dispatch_wgrad<__nv_bfloat16>(bn, smallc, a_tma, tma_red, tx, tdy, tdw, g, dw, st);
-  set_error("conv2d_wgrad_tc: unknown dtype %d", dtype);
-  return SIMCLR_ERR_INVALID_ARG;
+  if (!rc) rc = dispatch_wgrad<__nv_bfloat16>(bn, smallc, a_tma, tma_red, tx, tdy, tdw, g, dw, st);
+  if (!rc) rc = run_sum_partials(g.ws, g.ws_stride, dw, dw_elems, g.splits, st);
+  const int rf = scratch_free(g.ws, st);
+  return rc ? rc : rf;
 }
 
 int simclr_conv2d_wgrad_tc(const void* x, const void* dy, float* dw, int dtype, int64_t N, int64_t H, int64_t W,
@@ -1321,7 +1296,7 @@ int simclr_conv2d_wgrad_tc(const void* x, const void* dy, float* dw, int dtype, 
 // ways, v = v0 + v1 + v2 (8 + 8 + 8 mantissa bits, exact to 2^-25 |v|), and a product a*b is taken as
 //   a0*b0 + (a0*b1 + a1*b0) + (a1*b1 + a0*b2 + a2*b0)
 // -- all terms down to 2^-16 relative; what is dropped is 2^-24 -- each an exact-product / fp32-accumulate
-// tcgen05 GEMM, summed in fp32 at L2 (TMA reduce-add).  A two-way split (three GEMMs) leaves 2^-17 per
+// tensor-core GEMM, summed in fp32 at L2 (TMA reduce-add).  A two-way split (three GEMMs) leaves 2^-17 per
 // operand: measured 1e-2 on the step's gradients, not enough for the 1e-3 bar.  This is the tensor-core
 // verification mode: fp32 storage, 1e-3 step parity with the fp32 reference.
 // ---------------------------------------------------------------------------

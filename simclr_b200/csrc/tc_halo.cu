@@ -1,4 +1,4 @@
-// 3x3 stride-1 convolutions (fprop and dgrad) with HALO REUSE on the tcgen05 engine
+// 3x3 stride-1 convolutions (fprop and dgrad) with HALO REUSE on the wgmma engine
 // (tf2/resnet.py:446-455: the 3x3 of every bottleneck; 64 channels at 56x56, 128 at 28x28).
 //
 // The implicit-GEMM kernel of tc_conv.cu fetches every input byte once per filter tap (nine TMA
@@ -8,15 +8,15 @@
 // [TR+2][W+2][64 ch] of 128-byte, 128B-swizzled pixel rows.  GEMM row v of the tile is the "virtual
 // pixel" (v / Wp, v % Wp) of a (W+2)-wide grid, so the A operand of tap (r, s) is the SAME slab seen
 // from pixel offset r*Wp + s: a K-major SWIZZLE_128B descriptor whose start address is shifted by
-// that many 128-byte rows (tcgen05 applies the swizzle to absolute shared-memory address bits;
-// scripts/probe_umma_shift.cu, profiles/r02_probe_umma_shift.txt).  The two virtual columns per row
+// that many 128-byte rows (the swizzle is applied to absolute shared-memory address bits, so the
+// slab stays 1024-byte aligned and only the start moves).  The two virtual columns per row
 // that fall outside the image are computed and dropped (zeroed in the staging tile so the fused
 // BatchNorm statistics ignore them; clipped by the TMA store).  With 64 input channels the whole
 // filter (73 KB) stays resident in shared memory; wider layers stream it through a ring.
 //
-//   warps 0-3  epilogue   TMEM -> bf16 -> 128B-swizzled staging tile -> TMA store (+ column sums)
-//   warp  4    MMA issuer 9 taps x CB channel blocks x 4 tcgen05.mma (M128, N=BN, K16) per tile
-//   warp  5    TMA        slab loads (4-D tiled boxes), filter tiles
+//   warps 0-3  consumer   9 taps x CB channel blocks x 4 K16 steps x two m64 wgmmas (N=BN) per tile, then
+//                         registers -> bf16 -> 128B-swizzled staging tile -> TMA store (+ column sums)
+//   warp  4    TMA        slab loads (4-D tiled boxes), filter tiles
 #include "tc_common.cuh"
 
 namespace simclr {
@@ -41,7 +41,6 @@ template <int BN, int CB, bool B_RES> struct HaloCfg {
   static constexpr int SLAB_STAGE_BYTES = CB * SLAB_BYTES;
   static constexpr int B_TILE = BN * 128;                       // one (tap, channel block) filter tile
   static constexpr int B_STAGES = B_RES ? 9 * CB : 4;
-  static constexpr int TMEM_COLS = 2 * BN < 32 ? 32 : 2 * BN;
   static constexpr size_t SMEM = 1024 + (size_t)SLAB_STAGES * SLAB_STAGE_BYTES + (size_t)B_STAGES * B_TILE + 2 * EPI_TILE + 512;
 };
 
@@ -56,21 +55,17 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* tmap, const void
                ::"l"((uint64_t)tmap), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
-__device__ __forceinline__ void sts16h(uint32_t saddr, uint4 v) {
-  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
 __device__ __forceinline__ void warp_arrive_h(uint64_t* bar) {
   __syncwarp();
   if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
 }
 
 template <int BN, int CB, bool B_RES, bool STATS>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(160, 1)
 halo3x3_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                const __grid_constant__ CUtensorMap tmap_y, const HaloGeom g, double* __restrict__ bn_sums) {
   using CFG = HaloCfg<BN, CB, B_RES>;
   constexpr int SS = CFG::SLAB_STAGES, BS = CFG::B_STAGES;
-  constexpr uint32_t IDESC = make_idesc(false, 128, BN, false, false);
   constexpr int BOXES = BN / 64;
 
   extern __shared__ uint8_t smem_raw[];
@@ -83,65 +78,85 @@ halo3x3_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant
   uint64_t* slab_empty = bars + SS;        // [SS]
   uint64_t* b_full = bars + 2 * SS;        // [BS]  (resident filter: b_full[0] only, completes once)
   uint64_t* b_empty = b_full + BS;         // [BS]
-  uint64_t* tmem_full = b_empty + BS;      // [2]
-  uint64_t* tmem_empty = tmem_full + 2;    // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < SS; ++s) { mbar_init(&slab_full[s], 1); mbar_init(&slab_empty[s], 1); }
-    for (int s = 0; s < BS; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], 4); }
+    for (int s = 0; s < SS; ++s) { mbar_init(&slab_full[s], 1); mbar_init(&slab_empty[s], 4); }
+    for (int s = 0; s < BS; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 4); }
     fence_barrier_init();
   }
-  if (warp == 5 && lane == 0) { tma_prefetch_desc(&tmap_x); tma_prefetch_desc(&tmap_w); tma_prefetch_desc(&tmap_y); }
-  if (warp == 4) tmem_alloc(tmem_ptr, CFG::TMEM_COLS);
-  tc_fence_before();
+  if (warp == 4 && lane == 0) { tma_prefetch_desc(&tmap_x); tma_prefetch_desc(&tmap_w); tma_prefetch_desc(&tmap_y); }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp < 4) {
-    // ------------------------------ epilogue ------------------------------
-    int as = 0; uint32_t aphase = 0;
+    // ------------------------------ consumer: MMA + epilogue ------------------------------
+    // descriptor low words are running warp-uniform 32-bit sums; m64 half h is 64 virtual pixels further
+    constexpr uint32_t HI = desc_hi_sw128(1024);
+    int ss = 0; uint32_t sphase = 0;
+    int bs = 0; uint32_t bphase = 0;
+    const uint32_t slab0_lo = uniform_u32(desc_lo(smem_u32(slab), 16));
+    const uint32_t bt_lo = uniform_u32(desc_lo(smem_u32(bt), 16));
+    float acc[2][BN / 2];
     uint32_t box_ctr = 0;
-    const int row = warp * 32 + lane;                 // virtual pixel of this thread
-    const int vi = row / g.Wp, vj = row - vi * g.Wp;
+    bool rows_in[2][2];                                 // the thread's accumulator rows: virtual pixel inside the image
     const int sj = threadIdx.x & 7, srg = threadIdx.x >> 3;
     float st_sum[BOXES][8], st_sq[BOXES][8];
 #pragma unroll
     for (int b = 0; b < BOXES; ++b)
 #pragma unroll
       for (int c = 0; c < 8; ++c) { st_sum[b][c] = 0.f; st_sq[b][c] = 0.f; }
+    if (B_RES) { mbar_wait(&b_full[0], 0); }
     for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
       const int n = tile / g.tiles_per_img, p0 = (tile - n * g.tiles_per_img) * g.TR;
-      const bool valid = vi < g.TR && vj < g.W && p0 + vi < g.H;
-      mbar_wait(&tmem_full[as], aphase, 110);
-      tc_fence_after();
-      const uint32_t tbase = tmem_base + (uint32_t)(as * BN) + ((uint32_t)(warp * 32) << 16);
-#pragma unroll 1
+      mbar_wait(&slab_full[ss], sphase);
+      const uint32_t a_tile_lo = slab0_lo + (uint32_t)ss * (CFG::SLAB_STAGE_BYTES >> 4) + (uint32_t)g.tap_base * 8u;
+      int prev_bs = 0;
+#pragma unroll
+      for (int t = 0; t < 9; ++t) {
+        const int r = t / 3, sx = t % 3;
+        const uint32_t a_tap_lo = a_tile_lo + (uint32_t)(g.tap_sign * (r * g.Wp + sx)) * 8u;   // 128 B per pixel
+#pragma unroll
+        for (int cb = 0; cb < CB; ++cb) {
+          uint32_t b_lo;
+          if (B_RES) {
+            b_lo = bt_lo + (uint32_t)(t * CB + cb) * (CFG::B_TILE >> 4);
+          } else {
+            mbar_wait(&b_full[bs], bphase);
+            b_lo = bt_lo + (uint32_t)bs * (CFG::B_TILE >> 4);
+          }
+          const uint32_t a_lo = a_tap_lo + cb * (SLAB_BYTES >> 4);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              wgmma<BN, false, false, false>(acc[h], desc_pack(a_lo + h * (64 * 128 >> 4) + 2 * k, HI), desc_pack(b_lo + 2 * k, HI),
+                                             (t | cb | k) != 0 ? 1u : 0u);
+          wgmma_commit();
+          if (!B_RES) {
+            if (t | cb) { wgmma_wait<1>(); warp_arrive_h(&b_empty[prev_bs]); }
+            prev_bs = bs;
+            if (++bs == BS) { bs = 0; bphase ^= 1; }
+          }
+        }
+      }
+      wgmma_wait<0>(acc);
+      if (!B_RES) warp_arrive_h(&b_empty[prev_bs]);
+      warp_arrive_h(&slab_empty[ss]);
+      if (++ss == SS) { ss = 0; sphase ^= 1; }
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int rp = 0; rp < 2; ++rp) {
+          const int row = frag_row(h, rp), vi = row / g.Wp, vj = row - vi * g.Wp;
+          rows_in[h][rp] = vi < g.TR && vj < g.W && p0 + vi < g.H;      // outside the image: stored as zeros
+        }
+#pragma unroll
       for (int b = 0; b < BOXES; ++b, ++box_ctr) {
         uint8_t* stage = epi + (box_ctr & 1) * EPI_TILE;
         if (threadIdx.x == 0) tma_store_wait_read<1>();     // the store issued two boxes ago has read its tile
         named_barrier_sync(1, 128);
-        const uint32_t srow = smem_u32(stage);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          uint32_t acc[32];
-          tmem_ld32(tbase + b * 64 + h * 32, acc);
-          tmem_ld_wait();
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint32_t w[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              __nv_bfloat162 hh = __floats2bfloat162_rn(__uint_as_float(acc[8 * q + 2 * e]), __uint_as_float(acc[8 * q + 2 * e + 1]));
-              w[e] = valid ? *reinterpret_cast<uint32_t*>(&hh) : 0u;      // virtual pixels outside the image: zeros
-            }
-            sts16h(srow + sw128_offset(row, h * 4 + q), make_uint4(w[0], w[1], w[2], w[3]));
-          }
-        }
-        if (b == BOXES - 1) { tc_fence_before(); warp_arrive_h(&tmem_empty[as]); }
+        stage_frag<__nv_bfloat16>(smem_u32(stage), acc, b * 8, rows_in);
         fence_proxy_async();
         named_barrier_sync(1, 128);
         if (threadIdx.x == 0) { tma_store_4d(&tmap_y, stage, b * 64, 0, p0, n); tma_store_commit(); }
@@ -161,14 +176,9 @@ halo3x3_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant
             }
           }
 #pragma unroll
-          for (int bb = 0; bb < BOXES; ++bb)
-            if (bb == b) {
-#pragma unroll
-              for (int c = 0; c < 8; ++c) { st_sum[bb][c] += a0[c]; st_sq[bb][c] += a1[c]; }
-            }
+          for (int c = 0; c < 8; ++c) { st_sum[b][c] += a0[c]; st_sq[b][c] += a1[c]; }
         }
       }
-      as ^= 1; if (as == 0) aphase ^= 1;
     }
     if (STATS) {
       // Fold the row groups of a warp by shuffles, the four warps through shared memory (the slab ring is
@@ -192,63 +202,12 @@ halo3x3_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant
           double s0 = 0.0, s1 = 0.0;
 #pragma unroll
           for (int w = 0; w < 4; ++w) { s0 += (double)red[(w * BN + lc) * 2]; s1 += (double)red[(w * BN + lc) * 2 + 1]; }
-          atomicAdd(bn_sums + lc, s0);
-          atomicAdd(bn_sums + g.n_out + lc, s1);
+          bn_sums[(size_t)blockIdx.x * 2 * g.n_out + lc] = s0;            // this CTA's partial (added in CTA order)
+          bn_sums[(size_t)blockIdx.x * 2 * g.n_out + g.n_out + lc] = s1;
         }
       }
     }
     if (threadIdx.x == 0) tma_store_wait_all<0>();
-  } else if (warp == 4) {
-    // ------------------------------ MMA issuer ----------------------------
-    // Every lane runs the loop on warp-uniform values (descriptor low words are running 32-bit sums in
-    // uniform registers); only the tcgen05 instructions are predicated on lane 0.  The first version built
-    // each 64-bit descriptor from an address inside `if (lane == 0)`: ~20 SASS instructions and a local-memory
-    // load per MMA, ~130 cycles against the 32-48 cycles an M128 x N64 x K16 MMA takes -- the tensor pipe sat
-    // at 13 % (profiles/r02_ncu_halo.txt).
-    constexpr uint32_t HI = desc_hi_sw128(1024);
-    int ss = 0; uint32_t sphase = 0;
-    int bs = 0; uint32_t bphase = 0;
-    int as = 0; uint32_t aphase = 0;
-    const uint32_t slab0_lo = uniform_u32(desc_lo(smem_u32(slab), 16));
-    const uint32_t bt_lo = uniform_u32(desc_lo(smem_u32(bt), 16));
-    const uint32_t tmem_u = uniform_u32(tmem_base);
-    if (B_RES) { mbar_wait(&b_full[0], 0, 120); }
-    for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-      mbar_wait(&tmem_empty[as], aphase ^ 1, 121);
-      mbar_wait(&slab_full[ss], sphase, 122);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_u + (uint32_t)(as * BN);
-      const uint32_t a_tile_lo = slab0_lo + (uint32_t)ss * (CFG::SLAB_STAGE_BYTES >> 4) + (uint32_t)g.tap_base * 8u;
-#pragma unroll
-      for (int t = 0; t < 9; ++t) {
-        const int r = t / 3, sx = t % 3;
-        const uint32_t a_tap_lo = a_tile_lo + (uint32_t)(g.tap_sign * (r * g.Wp + sx)) * 8u;   // 128 B per pixel
-#pragma unroll
-        for (int cb = 0; cb < CB; ++cb) {
-          uint32_t b_lo;
-          if (B_RES) {
-            b_lo = bt_lo + (uint32_t)(t * CB + cb) * (CFG::B_TILE >> 4);
-          } else {
-            mbar_wait(&b_full[bs], bphase, 123);
-            tc_fence_after();
-            b_lo = bt_lo + (uint32_t)bs * (CFG::B_TILE >> 4);
-          }
-          const uint32_t a_lo = a_tap_lo + cb * (SLAB_BYTES >> 4);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma<false>(d_tmem, desc_pack(a_lo + 2 * k, HI), desc_pack(b_lo + 2 * k, HI), IDESC, (t | cb | k) != 0 ? 1u : 0u);
-            if (!B_RES) umma_commit(&b_empty[bs]);
-          }
-          __syncwarp();
-          if (!B_RES) { if (++bs == BS) { bs = 0; bphase ^= 1; } }
-        }
-      }
-      if (elect_one()) { umma_commit(&slab_empty[ss]); umma_commit(&tmem_full[as]); }
-      __syncwarp();
-      if (++ss == SS) { ss = 0; sphase ^= 1; }
-      as ^= 1; if (as == 0) aphase ^= 1;
-    }
   } else {
     // ------------------------------ TMA producer --------------------------
     if (lane == 0) {
@@ -262,7 +221,7 @@ halo3x3_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant
       int bs = 0; uint32_t bphase = 0;
       auto load_slab = [&](int tile) {
         const int n = tile / g.tiles_per_img, p0 = (tile - n * g.tiles_per_img) * g.TR;
-        mbar_wait(&slab_empty[ss], sphase ^ 1, 130);
+        mbar_wait(&slab_empty[ss], sphase ^ 1);
         mbar_arrive_expect_tx(&slab_full[ss], CB * g.box_bytes);
         for (int cb = 0; cb < CB; ++cb)
           tma_load_4d(slab + (size_t)ss * CFG::SLAB_STAGE_BYTES + cb * SLAB_BYTES, &tmap_x, &slab_full[ss], cb * 64, -1, p0 - 1, n);
@@ -275,7 +234,7 @@ halo3x3_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant
         if (!B_RES) {
           for (int t = 0; t < 9; ++t)
             for (int cb = 0; cb < CB; ++cb) {
-              mbar_wait(&b_empty[bs], bphase ^ 1, 131);
+              mbar_wait(&b_empty[bs], bphase ^ 1);
               mbar_arrive_expect_tx(&b_full[bs], CFG::B_TILE);
               tma_load_2d(bt + (size_t)bs * CFG::B_TILE, &tmap_w, &b_full[bs], t * g.C + cb * 64, 0);
               if (++bs == BS) { bs = 0; bphase ^= 1; }
@@ -286,136 +245,119 @@ halo3x3_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant
     __syncwarp();
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (warp == 4) { tc_fence_after(); tmem_dealloc(tmem_base, CFG::TMEM_COLS); }
 }
 
 // ===========================================================================
 // wgrad of the 64 -> 64 channel 3x3 layers with halo reuse.
 //   dW[(r,s,c)][co] = sum over pixels  X[pixel + (r,s)][c] * dY[pixel][co]
 // Both operands are MN-major (the reduction K runs over pixels, rows of 128 bytes): the X slab of a tile is the
-// fprop slab, tap (r, s) is the slab shifted by r*Wp + s rows along K, and TWO taps share one M = 128 operand --
-// the second 64-channel atom sits LBO = (offset difference) * 128 bytes after the first, i.e. the atoms overlap in
-// shared memory (scripts/probe_umma_mn_shift.cu: tcgen05 takes any 128-byte multiple for the start and for LBO).
-// Five accumulators [128 x 64] (tap pairs (0,1) (2,3) (4,5) (6,7) (8,8)) live in TMEM for the whole kernel: every
-// CTA sweeps its tiles, then adds its [576 x 64] partial into dW with TMA reduce-add.  The generic wgrad kernel
-// re-fetches X once per tap and dY once per 128 filter rows: 120 KB of L2 -> SM traffic per 64 pixels against
-// 24 KB here.  dY columns outside the image arrive as zeros (TMA out-of-bounds fill), buffer rows the boxes never
-// write are zeroed once, so virtual pixels contribute nothing.
+// fprop slab, and tap (r, s) is the slab shifted by r*Wp + s rows along K -- an M = 64 operand whose start is any
+// 128-byte row of the 1024-byte-aligned slab.  Nine accumulators [64 x 64] (one per tap) live in registers for the
+// whole kernel, three per consumer warpgroup: every CTA sweeps its tiles, then TMA-stores its [576 x 64] partial to
+// its rows of a scratch buffer, and run_sum_partials adds the CTAs' partials into dW in CTA order.  The generic wgrad kernel re-fetches X once per tap and dY once per 128 filter rows: 120 KB of
+// L2 -> SM traffic per 64 pixels against 24 KB here.  dY columns outside the image arrive as zeros (TMA
+// out-of-bounds fill), buffer rows the boxes never write are zeroed once, so virtual pixels contribute nothing.
+//
+//   warps 0-11  consumers  warpgroup w owns taps 3w .. 3w + 2
+//   warp  12    TMA        X slab and dY boxes
 // ===========================================================================
 constexpr int WG_DY_BYTES = 128 * 128;                       // [128 virtual pixels][64 co]
 constexpr int WG_STAGE_BYTES = SLAB_BYTES + WG_DY_BYTES;     // 48 KB
 constexpr int WG_STAGES = 3;
-constexpr size_t WG_SMEM = 1024 + (size_t)WG_STAGES * WG_STAGE_BYTES + 2 * EPI_TILE + 256;
+constexpr int WG_GROUPS = 3;                                 // consumer warpgroups
+constexpr int WG_EPI_TILE = 64 * 128;                        // [64 filter rows][32 fp32]
+constexpr size_t WG_SMEM = 1024 + (size_t)WG_STAGES * WG_STAGE_BYTES + WG_GROUPS * 2 * WG_EPI_TILE + 256;
 
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(WG_GROUPS * 128 + 32, 1)
 halo3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_dy,
                      const __grid_constant__ CUtensorMap tmap_dw, const HaloGeom g) {
-  constexpr uint32_t IDESC = make_idesc(false, 128, 64, true, true);
   constexpr uint32_t HI = desc_hi_sw128(1024);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* epi = smem + (size_t)WG_STAGES * WG_STAGE_BYTES;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(epi + 2 * EPI_TILE);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(epi + WG_GROUPS * 2 * WG_EPI_TILE);
   uint64_t* full = bars;                     // [WG_STAGES]
   uint64_t* empty = bars + WG_STAGES;        // [WG_STAGES]
-  uint64_t* acc_full = empty + WG_STAGES;    // [1]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_full + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   // zero the operand ring once: the TMA boxes never write the tail rows, and 0 * stale NaN would poison the sums
   for (int i = threadIdx.x; i < WG_STAGES * WG_STAGE_BYTES / 16; i += blockDim.x)
     reinterpret_cast<uint4*>(smem)[i] = make_uint4(0u, 0u, 0u, 0u);
   if (threadIdx.x == 0) {
-    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(acc_full, 1);
+    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], WG_GROUPS * 4); }
     fence_barrier_init();
   }
   fence_proxy_async();
-  if (warp == 5 && lane == 0) { tma_prefetch_desc(&tmap_x); tma_prefetch_desc(&tmap_dy); tma_prefetch_desc(&tmap_dw); }
-  if (warp == 4) tmem_alloc(tmem_ptr, 512);
-  tc_fence_before();
+  if (warp == WG_GROUPS * 4 && lane == 0) { tma_prefetch_desc(&tmap_x); tma_prefetch_desc(&tmap_dy); tma_prefetch_desc(&tmap_dw); }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   const bool has_work = (int)blockIdx.x < g.num_tiles;
 
-  if (warp < 4) {
-    // ------------------------------ epilogue (once) ------------------------------
-    if (has_work) {
-      mbar_wait(acc_full, 0, 210);
-      tc_fence_after();
-      const int row = warp * 32 + lane;
-      uint32_t box_ctr = 0;
-#pragma unroll 1
-      for (int pr = 0; pr < 5; ++pr) {
-#pragma unroll 1
-        for (int cc = 0; cc < 2; ++cc, ++box_ctr) {
-          uint8_t* stage = epi + (box_ctr & 1) * EPI_TILE;
-          if (threadIdx.x == 0) tma_store_wait_read<1>();
-          named_barrier_sync(1, 128);
-          uint32_t acc[32];
-          tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + pr * 64 + cc * 32, acc);
-          tmem_ld_wait();
-          const uint32_t srow = smem_u32(stage);
-#pragma unroll
-          for (int q = 0; q < 8; ++q)
-            sts16h(srow + sw128_offset(row, q), make_uint4(acc[4 * q], acc[4 * q + 1], acc[4 * q + 2], acc[4 * q + 3]));
-          fence_proxy_async();
-          named_barrier_sync(1, 128);
-          // rows of accumulator `pr` are filter rows [pr*128, pr*128 + 128) of the [9*64][64] matrix; the duplicate
-          // tap of the last pair lands at rows >= 576 and is clipped by the tensor map
-          if (threadIdx.x == 0) { tma_reduce_add_2d(&tmap_dw, stage, cc * 32, pr * 128); tma_store_commit(); }
-        }
-      }
-      if (threadIdx.x == 0) tma_store_wait_all<0>();
-    }
-  } else if (warp == 4) {
-    // ------------------------------ MMA issuer ----------------------------
+  if (warp < WG_GROUPS * 4) {
+    // ------------------------------ consumers ------------------------------
+    const int wg = warp >> 2, wt = threadIdx.x & 127;
     int ss = 0; uint32_t sphase = 0;
-    const uint32_t smem_lo = uniform_u32((smem_u32(smem) & 0x3FFFFu) >> 4);
-    const uint32_t tmem_u = uniform_u32(tmem_base);
+    const uint32_t smem_lo = uniform_u32(desc_lo(smem_u32(smem), 1024));
     const int Wp = g.Wp;
+    uint32_t off[3];                                      // slab row of tap 3*wg + j (128 B per row)
+#pragma unroll
+    for (int j = 0; j < 3; ++j) { const int t = 3 * wg + j; off[j] = (uint32_t)((t / 3) * Wp + t % 3) * 8u; }
+    float acc[3][32];
     bool first = true;
     for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-      mbar_wait(&full[ss], sphase, 220);
-      tc_fence_after();
+      mbar_wait(&full[ss], sphase);
       const uint32_t x_lo = smem_lo + (uint32_t)ss * (WG_STAGE_BYTES >> 4);
       const uint32_t dy_lo = x_lo + (SLAB_BYTES >> 4);
-      if (elect_one()) {
-        // K step outermost, the five accumulators innermost: consecutive MMAs never accumulate into the same columns
-        // (for the stem's small M64 x N32 MMAs that order was worth 1.29 -> 0.72 ms; here 0.81 -> 0.76 ms)
-        uint32_t a_lo[5];
+      wgmma_fence();
+      // K step outermost, the three accumulators innermost: consecutive MMAs never accumulate into the same registers
 #pragma unroll
-        for (int pr = 0; pr < 5; ++pr) {
-          const int ta = 2 * pr, tb = pr == 4 ? 8 : 2 * pr + 1;
-          const int offa = (ta / 3) * Wp + ta % 3, offb = (tb / 3) * Wp + tb % 3;
-          a_lo[pr] = (x_lo + (uint32_t)offa * 8u) | ((((uint32_t)(offb - offa) * 8u) & 0x3FFFu) << 16);   // LBO = (offb - offa) * 128 B
-        }
-        const uint32_t b_lo = dy_lo | (1u << 16);
+      for (int k = 0; k < 8; ++k) {        // 16 pixels (16 rows of 128 B) per MMA
+        const uint64_t bd = desc_pack(dy_lo + k * 128, HI);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) {        // 16 pixels (16 rows of 128 B) per MMA
-          const uint64_t bd = desc_pack(b_lo + k * 128, HI);
-#pragma unroll
-          for (int pr = 0; pr < 5; ++pr)
-            umma<false>(tmem_u + pr * 64, desc_pack(a_lo[pr] + k * 128, HI), bd, IDESC, (!first || k > 0) ? 1u : 0u);
-        }
-        umma_commit(&empty[ss]);
+        for (int j = 0; j < 3; ++j)
+          wgmma<64, false, true, true>(acc[j], desc_pack(x_lo + off[j] + k * 128, HI), bd, (!first || k > 0) ? 1u : 0u);
       }
-      __syncwarp();
+      wgmma_commit();
+      wgmma_wait<0>(acc);
+      warp_arrive_h(&empty[ss]);
       first = false;
       if (++ss == WG_STAGES) { ss = 0; sphase ^= 1; }
     }
-    if (has_work && elect_one()) umma_commit(acc_full);
-    __syncwarp();
+    // ------------------------------ epilogue (once) ------------------------------
+    if (has_work) {
+      const int q = lane & 3;
+      uint32_t box_ctr = 0;
+#pragma unroll
+      for (int j = 0; j < 3; ++j) {
+#pragma unroll
+        for (int cc = 0; cc < 2; ++cc, ++box_ctr) {
+          uint8_t* stage = epi + (size_t)(wg * 2 + (box_ctr & 1)) * WG_EPI_TILE;
+          if (wt == 0) tma_store_wait_read<1>();
+          named_barrier_sync(1 + wg, 128);
+          const uint32_t srow = smem_u32(stage);
+#pragma unroll
+          for (int rp = 0; rp < 2; ++rp) {
+            const int row = 16 * (warp & 3) + (lane >> 2) + 8 * rp;
+#pragma unroll
+            for (int ii = 0; ii < 4; ++ii)
+              asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(srow + sw128_offset(row, 2 * ii + (q >> 1)) + 8 * (q & 1)),
+                           "f"(acc[j][4 * (4 * cc + ii) + 2 * rp]), "f"(acc[j][4 * (4 * cc + ii) + 2 * rp + 1]) : "memory");
+          }
+          fence_proxy_async();
+          named_barrier_sync(1 + wg, 128);
+          // rows of tap t are filter rows [t*64, t*64 + 64) of this CTA's [9*64][64] partial
+          if (wt == 0) { tma_store_2d(&tmap_dw, stage, cc * 32, (int)blockIdx.x * 576 + (3 * wg + j) * 64); tma_store_commit(); }
+        }
+      }
+      if (wt == 0) tma_store_wait_all<0>();
+    }
   } else {
     // ------------------------------ TMA producer --------------------------
     if (lane == 0) {
       int ss = 0; uint32_t sphase = 0;
       for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
         const int n = tile / g.tiles_per_img, p0 = (tile - n * g.tiles_per_img) * g.TR;
-        mbar_wait(&empty[ss], sphase ^ 1, 230);
+        mbar_wait(&empty[ss], sphase ^ 1);
         uint8_t* st = smem + (size_t)ss * WG_STAGE_BYTES;
         mbar_arrive_expect_tx(&full[ss], g.box_bytes + g.TR * g.Wp * 128);
         tma_load_4d(st, &tmap_x, &full[ss], 0, -1, p0 - 1, n);
@@ -426,9 +368,7 @@ halo3x3_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
     __syncwarp();
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (warp == 4) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
 }
 
 // rank-4 tiled map over an NHWC tensor {C, W, H, N}, boxes {64 channels, bw, bh, 1}, 128B swizzle, zero fill
@@ -459,7 +399,7 @@ int launch_halo(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap&
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CFG::SMEM);
   if (e != cudaSuccess) { set_error("halo3x3: cudaFuncSetAttribute(smem=%zu): %s", CFG::SMEM, cudaGetErrorString(e)); return (int)e; }
   int grid = g.num_tiles < num_sms() ? g.num_tiles : num_sms();
-  kern<<<grid, 192, CFG::SMEM, st>>>(tx, tw, ty, g, bn_sums);
+  kern<<<grid, 160, CFG::SMEM, st>>>(tx, tw, ty, g, bn_sums);
   SIMCLR_CHECK_LAUNCH();
   return SIMCLR_OK;
 }
@@ -510,10 +450,19 @@ int run_halo3x3(int mode, const void* src, const void* wk, void* out, int64_t N,
     cudaError_t e = cudaMemsetAsync(bn_sums, 0, 2 * (size_t)n_out * sizeof(double), st);
     if (e != cudaSuccess) { set_error("halo3x3: memset: %s", cudaGetErrorString(e)); return (int)e; }
   }
-  if (C == 64) return bn_sums ? launch_halo<64, 1, true, true>(tx, tw, ty, g, bn_sums, st)
-                              : launch_halo<64, 1, true, false>(tx, tw, ty, g, nullptr, st);
-  return bn_sums ? launch_halo<128, 2, false, true>(tx, tw, ty, g, bn_sums, st)
-                 : launch_halo<128, 2, false, false>(tx, tw, ty, g, nullptr, st);
+  if (!bn_sums) return C == 64 ? launch_halo<64, 1, true, false>(tx, tw, ty, g, nullptr, st)
+                                : launch_halo<128, 2, false, false>(tx, tw, ty, g, nullptr, st);
+  // fused statistics: one [2][n_out] partial per CTA, added into bn_sums in CTA order
+  const int nparts = num_sms();
+  double* parts = nullptr;
+  rc = scratch_alloc(&parts, (size_t)nparts * 2 * n_out * sizeof(double), st);
+  if (rc) return rc;
+  const cudaError_t e = cudaMemsetAsync(parts, 0, (size_t)nparts * 2 * n_out * sizeof(double), st);
+  if (e != cudaSuccess) { set_error("halo3x3: memset: %s", cudaGetErrorString(e)); scratch_free(parts, st); return (int)e; }
+  rc = C == 64 ? launch_halo<64, 1, true, true>(tx, tw, ty, g, parts, st) : launch_halo<128, 2, false, true>(tx, tw, ty, g, parts, st);
+  if (!rc) rc = run_sum_partials_f64(parts, 2 * n_out, bn_sums, 2 * n_out, nparts, st);
+  const int rf = scratch_free(parts, st);
+  return rc ? rc : rf;
 }
 
 bool halo3x3_wgrad_applicable(int dtype, int64_t N, int64_t H, int64_t W, int64_t Cs, int64_t Cin, int64_t Cout, int64_t R,
@@ -538,20 +487,26 @@ int run_halo3x3_wgrad(const void* x, const void* dy, float* dw, int64_t N, int64
   g.H = (int)H; g.W = (int)W; g.Wp = (int)W + 2; g.TR = 128 / g.Wp; g.N = (int)N;
   g.tiles_per_img = (int)((H + g.TR - 1) / g.TR); g.num_tiles = (int)(N * g.tiles_per_img);
   g.box_bytes = (g.TR + 2) * g.Wp * 128; g.n_out = 64; g.C = 64; g.tap_base = 0; g.tap_sign = 1;
+  const int grid = g.num_tiles < num_sms() ? g.num_tiles : num_sms();
   CUtensorMap tx, tdy, tdw;
   int rc = make_tmap_nhwc_tiled(&tx, x, (uint64_t)N, (uint64_t)H, (uint64_t)W, 64, (uint32_t)g.Wp, (uint32_t)(g.TR + 2));
   if (rc) return rc;
   rc = make_tmap_nhwc_tiled(&tdy, dy, (uint64_t)N, (uint64_t)H, (uint64_t)W, 64, (uint32_t)g.Wp, (uint32_t)g.TR);
   if (rc) return rc;
-  rc = make_tmap_2d(&tdw, dw, 4, 9 * 64, 64, 64 * 4, 128, 32);
-  if (rc) return rc;
   if (zero && !accumulate_prezeroed()) SIMCLR_CHECK_CUDA(cudaMemsetAsync(dw, 0, (size_t)9 * 64 * 64 * sizeof(float), st));
+  float* ws = nullptr;                                      // [grid][576][64] per-CTA partials
+  rc = scratch_alloc(&ws, (size_t)grid * 576 * 64 * sizeof(float), st);
+  if (rc) return rc;
+  rc = make_tmap_2d(&tdw, ws, 4, (uint64_t)grid * 576, 64, 64 * 4, 64, 32);
+  if (rc) { scratch_free(ws, st); return rc; }
   cudaError_t e = cudaFuncSetAttribute(halo3x3_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM);
-  if (e != cudaSuccess) { set_error("halo3x3_wgrad: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return (int)e; }
-  const int grid = g.num_tiles < num_sms() ? g.num_tiles : num_sms();
-  halo3x3_wgrad_kernel<<<grid, 192, WG_SMEM, st>>>(tx, tdy, tdw, g);
-  SIMCLR_CHECK_LAUNCH();
-  return SIMCLR_OK;
+  if (e != cudaSuccess) { set_error("halo3x3_wgrad: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); scratch_free(ws, st); return (int)e; }
+  halo3x3_wgrad_kernel<<<grid, WG_GROUPS * 128 + 32, WG_SMEM, st>>>(tx, tdy, tdw, g);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) { set_error("halo3x3_wgrad: launch: %s", cudaGetErrorString(e)); scratch_free(ws, st); return (int)e; }
+  rc = run_sum_partials(ws, 576 * 64, dw, 576 * 64, grid, st);
+  const int rf = scratch_free(ws, st);
+  return rc ? rc : rf;
 }
 
 }  // namespace tc

@@ -1,5 +1,5 @@
 // The stem convolution (tf2/resnet.py:593-604: 7x7, stride 2, 3 -> 64*width channels on the 224x224 input) on the
-// tcgen05 engine WITHOUT an im2col copy.
+// wgmma engine WITHOUT an im2col copy.
 //
 // The generic kernel gathers every A row (one output pixel: 7 filter rows x 64 bytes) with cp.async from L2: 57 KB
 // per 128-pixel tile against 6 KB of distinct input -- the layer ran at 0.23 of its HBM roofline, bound by L2 -> SM
@@ -7,15 +7,14 @@
 // (4 stored channels: a "pair" = 2 pixels = 8 bf16 = 16 bytes; out-of-image pairs arrive as zeros).  For output pixel
 // q and filter row r the K run (8 column slots x 4 channels; slot 0 has zero weights, see simclr_pack_conv_weight) is
 // the 64 contiguous bytes starting at pair q of slab row r.  Neighbouring output pixels start ONE pair apart, so the
-// A operand of filter row r is a K-major, NON-swizzled UMMA operand whose 8-row x 16-byte core matrices overlap:
-// row pitch 16 B, leading (K) byte offset 16 B, stride (8-row group) byte offset 128 B, start = slab row r
-// (scripts/probe_umma_nosw_overlap.cu, profiles/r02_probe_umma_nosw_overlap.txt).  A tile is one output row: M = 128
-// GEMM rows of which Q are real (rows >= Q read stale shared memory and are dropped), 7 x 2 MMAs (M128, N=BN, K16).
-// The packed filter [BN][256] stays resident in shared memory; BatchNorm statistics are taken in the epilogue.
+// A operand of filter row r is a K-major, NON-swizzled wgmma operand whose 8-row x 16-byte core matrices overlap:
+// row pitch 16 B, leading (K) byte offset 16 B, stride (8-row group) byte offset 128 B, start = slab row r.  A tile
+// is one output row: M = 128 GEMM rows of which Q are real (rows >= Q read stale shared memory and are dropped),
+// 7 x 2 K16 steps x two m64 wgmmas (N=BN <= 128).  The packed filter [BN][256] stays resident in shared memory;
+// BatchNorm statistics are taken in the epilogue.
 //
-//   warps 0-3  epilogue   TMEM -> bf16 -> 128B-swizzled staging tile -> TMA store (+ column sums)
-//   warp  4    MMA issuer
-//   warp  5    TMA        slab loads (4-D tiled boxes), filter
+//   warps 0-3  consumer   MMAs, then registers -> bf16 -> 128B-swizzled staging tile -> TMA store (+ column sums)
+//   warp  4    TMA        slab loads (4-D tiled boxes), filter
 #include "tc_common.cuh"
 
 namespace simclr {
@@ -37,7 +36,6 @@ struct StemGeom7 {
 
 template <int BN> struct StemCfg {
   static constexpr int B_TILE = BN * 128;                          // one K block of the filter
-  static constexpr int TMEM_COLS = 2 * BN < 32 ? 32 : 2 * BN;
   static size_t smem(int slab_stage_bytes) {
     return 1024 + (size_t)ST_SLAB_STAGES * slab_stage_bytes + (size_t)ST_KB * B_TILE + 2 * ST_EPI_TILE + 256;
   }
@@ -49,21 +47,17 @@ __device__ __forceinline__ void st_tma_load_4d(void* smem_dst, const CUtensorMap
       ::"r"(smem_u32(smem_dst)), "l"((uint64_t)tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-__device__ __forceinline__ void st_sts16(uint32_t saddr, uint4 v) {
-  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ void st_warp_arrive(uint64_t* bar) {
+__device__ __forceinline__ void warp_arrive_st(uint64_t* bar) {
   __syncwarp();
   if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
 }
 
 template <int BN, bool STATS>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(160, 1)
 stem7x7_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                const __grid_constant__ CUtensorMap tmap_y, const StemGeom7 g, double* __restrict__ bn_sums) {
   using CFG = StemCfg<BN>;
   constexpr int SS = ST_SLAB_STAGES;
-  constexpr uint32_t IDESC = make_idesc(false, 128, BN, false, false);
   constexpr int BOXES = BN / 64;
 
   extern __shared__ uint8_t smem_raw[];
@@ -75,63 +69,65 @@ stem7x7_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant
   uint64_t* slab_full = bars;              // [SS]
   uint64_t* slab_empty = bars + SS;        // [SS]
   uint64_t* b_full = bars + 2 * SS;        // [1]
-  uint64_t* tmem_full = b_full + 1;        // [2]
-  uint64_t* tmem_empty = tmem_full + 2;    // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < SS; ++s) { mbar_init(&slab_full[s], 1); mbar_init(&slab_empty[s], 1); }
+    for (int s = 0; s < SS; ++s) { mbar_init(&slab_full[s], 1); mbar_init(&slab_empty[s], 4); }
     mbar_init(b_full, 1);
-    for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], 4); }
     fence_barrier_init();
   }
-  if (warp == 5 && lane == 0) { tma_prefetch_desc(&tmap_x); tma_prefetch_desc(&tmap_w); tma_prefetch_desc(&tmap_y); }
-  if (warp == 4) tmem_alloc(tmem_ptr, CFG::TMEM_COLS);
-  tc_fence_before();
+  if (warp == 4 && lane == 0) { tma_prefetch_desc(&tmap_x); tma_prefetch_desc(&tmap_w); tma_prefetch_desc(&tmap_y); }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp < 4) {
-    // ------------------------------ epilogue ------------------------------
-    int as = 0; uint32_t aphase = 0;
+    // ------------------------------ consumer: MMA + epilogue ------------------------------
+    // descriptor low words are running warp-uniform 32-bit values (see tc_halo.cu); A: no swizzle, LBO 16 B, SBO 128 B,
+    // m64 half h starts 64 pixel pairs (1024 B) further
+    constexpr uint32_t HI_B = desc_hi_sw128(1024);
+    constexpr uint32_t HI_A = desc_hi_none(128);
+    int ss = 0; uint32_t sphase = 0;
+    const uint32_t slab0_lo = uniform_u32(desc_lo(smem_u32(slab), 16));
+    const uint32_t bt_lo = uniform_u32(desc_lo(smem_u32(bt), 16));
+    const uint32_t stage16 = (uint32_t)(g.slab_stage_bytes >> 4), pitch16 = (uint32_t)g.box_pairs;
+    float acc[2][BN / 2];
     uint32_t box_ctr = 0;
-    const int row = warp * 32 + lane;                 // output pixel q of this thread
-    const bool valid = row < g.Q;
+    bool rows_in[2][2];                                 // output pixel q of the accumulator row exists
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int rp = 0; rp < 2; ++rp) rows_in[h][rp] = frag_row(h, rp) < g.Q;
     const int sj = threadIdx.x & 7, srg = threadIdx.x >> 3;
     float st_sum[BOXES][8], st_sq[BOXES][8];
 #pragma unroll
     for (int b = 0; b < BOXES; ++b)
 #pragma unroll
       for (int c = 0; c < 8; ++c) { st_sum[b][c] = 0.f; st_sq[b][c] = 0.f; }
+    mbar_wait(b_full, 0);
     for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-      mbar_wait(&tmem_full[as], aphase, 210);
-      tc_fence_after();
-      const uint32_t tbase = tmem_base + (uint32_t)(as * BN) + ((uint32_t)(warp * 32) << 16);
-#pragma unroll 1
+      mbar_wait(&slab_full[ss], sphase);
+      const uint32_t a_tile_lo = slab0_lo + (uint32_t)ss * stage16;
+      wgmma_fence();
+#pragma unroll
+      for (int r = 0; r < 7; ++r) {
+        const uint32_t a_lo = a_tile_lo + (uint32_t)r * pitch16;
+        const uint32_t b_lo = bt_lo + (uint32_t)(r >> 1) * (CFG::B_TILE >> 4) + (uint32_t)(r & 1) * 4u;
+#pragma unroll
+        for (int k = 0; k < 2; ++k)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            wgmma<BN, false, false, false>(acc[h], desc_pack(a_lo + h * 64 + 2 * k, HI_A), desc_pack(b_lo + 2 * k, HI_B),
+                                           (r | k) != 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>(acc);
+      warp_arrive_st(&slab_empty[ss]);
+      if (++ss == SS) { ss = 0; sphase ^= 1; }
+#pragma unroll
       for (int b = 0; b < BOXES; ++b, ++box_ctr) {
         uint8_t* stage = epi + (box_ctr & 1) * ST_EPI_TILE;
         if (threadIdx.x == 0) tma_store_wait_read<1>();     // the store issued two boxes ago has read its tile
         named_barrier_sync(1, 128);
-        const uint32_t srow = smem_u32(stage);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          uint32_t acc[32];
-          tmem_ld32(tbase + b * 64 + h * 32, acc);
-          tmem_ld_wait();
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint32_t w[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              __nv_bfloat162 hh = __floats2bfloat162_rn(__uint_as_float(acc[8 * q + 2 * e]), __uint_as_float(acc[8 * q + 2 * e + 1]));
-              w[e] = valid ? *reinterpret_cast<uint32_t*>(&hh) : 0u;      // GEMM rows beyond the image row: zeros
-            }
-            st_sts16(srow + sw128_offset(row, h * 4 + q), make_uint4(w[0], w[1], w[2], w[3]));
-          }
-        }
-        if (b == BOXES - 1) { tc_fence_before(); st_warp_arrive(&tmem_empty[as]); }
+        stage_frag<__nv_bfloat16>(smem_u32(stage), acc, b * 8, rows_in);   // GEMM rows beyond the image row: zeros
         fence_proxy_async();
         named_barrier_sync(1, 128);
         // output rows of this tile: pixels tile*Q .. tile*Q + Q - 1 of the [N*P*Q][n_out] view (the box is Q rows high)
@@ -152,21 +148,16 @@ stem7x7_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant
             }
           }
 #pragma unroll
-          for (int bb = 0; bb < BOXES; ++bb)
-            if (bb == b) {
-#pragma unroll
-              for (int c = 0; c < 8; ++c) { st_sum[bb][c] += a0[c]; st_sq[bb][c] += a1[c]; }
-            }
+          for (int c = 0; c < 8; ++c) { st_sum[b][c] += a0[c]; st_sq[b][c] += a1[c]; }
         }
       }
-      as ^= 1; if (as == 0) aphase ^= 1;
     }
     if (STATS) {
       // fold the row groups of a warp by shuffles, the four warps through shared memory (staging tile 0 is free once
       // its last store has been read), then ONE fp64 atomic per column per CTA
       if (threadIdx.x == 0) tma_store_wait_read<0>();
       named_barrier_sync(1, 128);
-      float* red = reinterpret_cast<float*>(epi);        // [4 warps][BN columns][2]  (<= 8 KB)
+      float* red = reinterpret_cast<float*>(epi);        // [4 warps][BN columns][2]  (<= 4 KB)
 #pragma unroll
       for (int b = 0; b < BOXES; ++b) {
 #pragma unroll
@@ -184,46 +175,12 @@ stem7x7_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant
           double s0 = 0.0, s1 = 0.0;
 #pragma unroll
           for (int w = 0; w < 4; ++w) { s0 += (double)red[(w * BN + lc) * 2]; s1 += (double)red[(w * BN + lc) * 2 + 1]; }
-          atomicAdd(bn_sums + lc, s0);
-          atomicAdd(bn_sums + g.n_out + lc, s1);
+          bn_sums[(size_t)blockIdx.x * 2 * g.n_out + lc] = s0;            // this CTA's partial (added in CTA order)
+          bn_sums[(size_t)blockIdx.x * 2 * g.n_out + g.n_out + lc] = s1;
         }
       }
     }
     if (threadIdx.x == 0) tma_store_wait_all<0>();
-  } else if (warp == 4) {
-    // ------------------------------ MMA issuer ----------------------------
-    // descriptor low words are running warp-uniform 32-bit values (see tc_halo.cu); A: no swizzle, LBO 16 B, SBO 128 B
-    constexpr uint32_t HI_B = desc_hi_sw128(1024);
-    constexpr uint32_t HI_A = ((128u >> 4) & 0x3FFFu) | (1u << 14);
-    int ss = 0; uint32_t sphase = 0;
-    int as = 0; uint32_t aphase = 0;
-    const uint32_t slab0_lo = uniform_u32(desc_lo(smem_u32(slab), 16));
-    const uint32_t bt_lo = uniform_u32(desc_lo(smem_u32(bt), 16));
-    const uint32_t tmem_u = uniform_u32(tmem_base);
-    const uint32_t stage16 = (uint32_t)(g.slab_stage_bytes >> 4), pitch16 = (uint32_t)g.box_pairs;
-    mbar_wait(b_full, 0, 220);
-    for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-      mbar_wait(&tmem_empty[as], aphase ^ 1, 221);
-      mbar_wait(&slab_full[ss], sphase, 222);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_u + (uint32_t)(as * BN);
-      const uint32_t a_tile_lo = slab0_lo + (uint32_t)ss * stage16;
-      if (elect_one()) {
-#pragma unroll
-        for (int r = 0; r < 7; ++r) {
-          const uint32_t a_lo = a_tile_lo + (uint32_t)r * pitch16;
-          const uint32_t b_lo = bt_lo + (uint32_t)(r >> 1) * (CFG::B_TILE >> 4) + (uint32_t)(r & 1) * 4u;
-#pragma unroll
-          for (int k = 0; k < 2; ++k)
-            umma<false>(d_tmem, desc_pack(a_lo + 2 * k, HI_A), desc_pack(b_lo + 2 * k, HI_B), IDESC, (r | k) != 0 ? 1u : 0u);
-        }
-        umma_commit(&slab_empty[ss]);
-        umma_commit(&tmem_full[as]);
-      }
-      __syncwarp();
-      if (++ss == SS) { ss = 0; sphase ^= 1; }
-      as ^= 1; if (as == 0) aphase ^= 1;
-    }
   } else {
     // ------------------------------ TMA producer --------------------------
     if (lane == 0) {
@@ -232,7 +189,7 @@ stem7x7_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant
       int ss = 0; uint32_t sphase = 0;
       for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
         const int n = tile / g.P, p = tile - n * g.P;
-        mbar_wait(&slab_empty[ss], sphase ^ 1, 230);
+        mbar_wait(&slab_empty[ss], sphase ^ 1);
         mbar_arrive_expect_tx(&slab_full[ss], g.box_bytes);
         // pairs -2 .. Q (column 2q - 4 + slot), rows 2p - 3 .. 2p + 3; everything outside the image is zero-filled
         st_tma_load_4d(slab + (size_t)ss * g.slab_stage_bytes, &tmap_x, &slab_full[ss], 0, -2, 2 * p - 3, n);
@@ -242,9 +199,7 @@ stem7x7_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant
     __syncwarp();
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (warp == 4) { tc_fence_after(); tmem_dealloc(tmem_base, CFG::TMEM_COLS); }
 }
 
 // ===========================================================================
@@ -253,9 +208,11 @@ stem7x7_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant
 //   A = dY tile [pixels][64 co]   MN-major, 128B-swizzled (M = 64 output channels, K = pixels), TMA box of Q rows
 //   B = slab row r                MN-major, NOT swizzled: 8 k' (16 B) x 8 pixels (16 B apart) core matrices; the next
 //                                 8 k' sit ONE pair further (16 B, overlapping), the next 8 pixels 128 B further
-// Seven accumulators [64 x 32] (one per filter row) live in TMEM for the whole kernel; every CTA sweeps its output
-// rows and adds its partial into dW [7][7][Cin][64] with fp32 atomics (9408 per CTA).  Operand buffers are zeroed
+// Seven accumulators [64 x 32] (one per filter row) live in registers for the whole kernel; every CTA sweeps its output
+// rows and stores its partial dW [7][7][Cin][64] to its slot of a scratch buffer; run_sum_partials adds the CTAs'
+// partials into dW in CTA order.  Operand buffers are zeroed
 // once: dY rows beyond Q stay zero (the TMA box never writes them), so padded pixels contribute nothing.
+//   warps 0-3  consumer (MMAs, then the partial)      warp 4  TMA
 // ===========================================================================
 constexpr int SWG_STAGES = 3;
 struct StemWGeom {
@@ -266,98 +223,80 @@ struct StemWGeom {
   int Cin;
 };
 
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(160, 1)
 stem7x7_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_dy,
-                     const StemWGeom g, float* __restrict__ dw) {
-  constexpr uint32_t IDESC = make_idesc(false, 64, 32, true, true);
+                     const StemWGeom g, float* __restrict__ ws) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)SWG_STAGES * g.stage_bytes);
   uint64_t* full = bars;                      // [SWG_STAGES]
   uint64_t* empty = bars + SWG_STAGES;        // [SWG_STAGES]
-  uint64_t* acc_full = empty + SWG_STAGES;    // [1]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_full + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   for (int i = threadIdx.x; i < SWG_STAGES * g.stage_bytes / 16; i += blockDim.x)
     reinterpret_cast<uint4*>(smem)[i] = make_uint4(0u, 0u, 0u, 0u);
   if (threadIdx.x == 0) {
-    for (int s = 0; s < SWG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(acc_full, 1);
+    for (int s = 0; s < SWG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4); }
     fence_barrier_init();
   }
   fence_proxy_async();
-  if (warp == 5 && lane == 0) { tma_prefetch_desc(&tmap_x); tma_prefetch_desc(&tmap_dy); }
-  if (warp == 4) tmem_alloc(tmem_ptr, 256);
-  tc_fence_before();
+  if (warp == 4 && lane == 0) { tma_prefetch_desc(&tmap_x); tma_prefetch_desc(&tmap_dy); }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   const bool has_work = (int)blockIdx.x < g.num_tiles;
 
   if (warp < 4) {
-    // ------------------------------ epilogue (once) ------------------------------
-    if (has_work) {
-      mbar_wait(acc_full, 0, 310);
-      tc_fence_after();
-      // an M = 64 accumulator keeps 16 rows per 32-lane TMEM sub-partition (lanes 0-15 of each warp's quarter)
-      const int co = warp * 16 + lane;
-      const bool act = lane < 16;
-#pragma unroll 1
-      for (int r = 0; r < 7; ++r) {
-        uint32_t acc[32];
-        tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + r * 32, acc);
-        tmem_ld_wait();
-        if (act) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const int sp = j >> 2, c = j & 3;                 // column slot (0: the zero slot), stored channel
-            if (sp >= 1 && c < g.Cin) atomicAdd(dw + ((size_t)((r * 7 + sp - 1) * g.Cin + c)) * 64 + co, __uint_as_float(acc[j]));
-          }
-        }
-      }
-    }
-  } else if (warp == 4) {
-    // ------------------------------ MMA issuer ----------------------------
+    // ------------------------------ consumer ------------------------------
     constexpr uint32_t HI_A = desc_hi_sw128(1024);
     // slab operand, MN-major without swizzle: SBO = stride between 8-k' core matrices (16 B, overlapping),
     // LBO = stride between 8-pixel groups (128 B) -- the roles are the reverse of the swizzled MN-major layouts
-    const uint32_t hi_b = uniform_u32(1u | (1u << 14));          // SBO field (16-byte units)
+    constexpr uint32_t HI_B = desc_hi_none(16);
     const uint32_t lbo_b = uniform_u32(8u << 16);                // LBO field
     int ss = 0; uint32_t sphase = 0;
     const uint32_t smem_lo = uniform_u32((smem_u32(smem) & 0x3FFFFu) >> 4);
-    const uint32_t tmem_u = uniform_u32(tmem_base);
     const uint32_t stage16 = (uint32_t)(g.stage_bytes >> 4), dy16 = (uint32_t)(g.dy_bytes >> 4), pitch16 = (uint32_t)g.box_pairs;
+    float acc[7][16];
     bool first = true;
     for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
-      mbar_wait(&full[ss], sphase, 320);
-      tc_fence_after();
+      mbar_wait(&full[ss], sphase);
       const uint32_t dy_lo = (smem_lo + (uint32_t)ss * stage16) | (1u << 16);
       const uint32_t x_lo = (smem_lo + (uint32_t)ss * stage16 + dy16) | lbo_b;
-      if (elect_one()) {
-        // K step outermost: consecutive MMAs go to seven DIFFERENT accumulators (no back-to-back dependence on one)
+      wgmma_fence();
+      // K step outermost: consecutive MMAs go to seven DIFFERENT accumulators (no back-to-back dependence on one)
 #pragma unroll 1
-        for (int ks = 0; ks < g.ksteps; ++ks) {       // 16 pixels per MMA: 16 dY rows of 128 B, 16 pairs of the slab row
-          const uint64_t ad = desc_pack(dy_lo + ks * 128, HI_A);
+      for (int ks = 0; ks < g.ksteps; ++ks) {       // 16 pixels per MMA: 16 dY rows of 128 B, 16 pairs of the slab row
+        const uint64_t ad = desc_pack(dy_lo + ks * 128, HI_A);
 #pragma unroll
-          for (int r = 0; r < 7; ++r)
-            umma<false>(tmem_u + r * 32, ad, desc_pack(x_lo + r * pitch16 + ks * 16, hi_b), IDESC, (!first || ks > 0) ? 1u : 0u);
-        }
-        umma_commit(&empty[ss]);
+        for (int r = 0; r < 7; ++r)
+          wgmma<32, false, true, true>(acc[r], ad, desc_pack(x_lo + r * pitch16 + ks * 16, HI_B), (!first || ks > 0) ? 1u : 0u);
       }
-      __syncwarp();
+      wgmma_commit();
+      wgmma_wait<0>(acc);
+      warp_arrive_st(&empty[ss]);
       first = false;
       if (++ss == SWG_STAGES) { ss = 0; sphase ^= 1; }
     }
-    if (has_work && elect_one()) umma_commit(acc_full);
-    __syncwarp();
+    // ------------------------------ epilogue (once) ------------------------------
+    if (has_work) {
+      float* dw = ws + (size_t)blockIdx.x * 49 * g.Cin * 64;
+      // acc[r][4*i + v]: output channel 16*warp + lane/4 + 8*(v >> 1), k' = 8*i + 2*(lane % 4) + (v & 1)
+#pragma unroll
+      for (int r = 0; r < 7; ++r) {
+#pragma unroll
+        for (int v = 0; v < 16; ++v) {
+          const int co = 16 * warp + (lane >> 2) + 8 * ((v & 3) >> 1);
+          const int j = 8 * (v >> 2) + 2 * (lane & 3) + (v & 1);
+          const int sp = j >> 2, c = j & 3;                 // column slot (0: the zero slot), stored channel
+          if (sp >= 1 && c < g.Cin) dw[((size_t)((r * 7 + sp - 1) * g.Cin + c)) * 64 + co] = acc[r][v];
+        }
+      }
+    }
   } else {
     // ------------------------------ TMA producer --------------------------
     if (lane == 0) {
       int ss = 0; uint32_t sphase = 0;
       for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
         const int n = tile / g.P, p = tile - n * g.P;
-        mbar_wait(&empty[ss], sphase ^ 1, 330);
+        mbar_wait(&empty[ss], sphase ^ 1);
         uint8_t* st = smem + (size_t)ss * g.stage_bytes;
         mbar_arrive_expect_tx(&full[ss], g.box_bytes + g.Q * 128);
         tma_load_2d(st, &tmap_dy, &full[ss], 0, tile * g.Q);
@@ -368,9 +307,7 @@ stem7x7_wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_co
     __syncwarp();
   }
 
-  tc_fence_before();
   __syncthreads();
-  if (warp == 4) { tc_fence_after(); tmem_dealloc(tmem_base, 256); }
 }
 
 // x [N][H][W][4] bf16 seen as [N][H][W/2][8]: 16-byte pixel pairs, no swizzle
@@ -400,7 +337,7 @@ int launch_stem(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap&
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) { set_error("stem7x7: cudaFuncSetAttribute(smem=%zu): %s", smem, cudaGetErrorString(e)); return (int)e; }
   const int grid = g.num_tiles < num_sms() ? g.num_tiles : num_sms();
-  kern<<<grid, 192, smem, st>>>(tx, tw, ty, g, bn_sums);
+  kern<<<grid, 160, smem, st>>>(tx, tw, ty, g, bn_sums);
   SIMCLR_CHECK_LAUNCH();
   return SIMCLR_OK;
 }
@@ -418,12 +355,11 @@ bool stem7x7_applicable(int dtype, int out_dtype, int64_t N, int64_t H, int64_t 
   static int en = -1;
   if (en < 0) { const char* e = getenv("SIMCLR_TC_STEM"); en = (e && e[0] == '0') ? 0 : 1; }
   if (!en || dtype != SIMCLR_BF16 || out_dtype != SIMCLR_BF16 || Cs != 4 || R != 7 || S != 7 || stride != 2) return false;
-  if (!(n_out == 64 || n_out == 128 || n_out == 256) || W % 2 || H % 2 || P != H / 2 || Q != W / 2) return false;
+  if (!(n_out == 64 || n_out == 128) || W % 2 || H % 2 || P != H / 2 || Q != W / 2) return false;
   if (Q < 8 || Q > 128 || Q + 3 > 256) return false;
   if (N * P >= (1ll << 31) / 128) return false;
   if (!aligned16(src) || !aligned16(wk) || !aligned16(out)) return false;
-  const size_t smem = n_out == 64 ? StemCfg<64>::smem(slab_stage_bytes(Q)) : n_out == 128 ? StemCfg<128>::smem(slab_stage_bytes(Q))
-                                                                                            : StemCfg<256>::smem(slab_stage_bytes(Q));
+  const size_t smem = n_out == 64 ? StemCfg<64>::smem(slab_stage_bytes(Q)) : StemCfg<128>::smem(slab_stage_bytes(Q));
   if (smem > 227 * 1024) return false;
   return get_encode_tiled() != nullptr;
 }
@@ -445,11 +381,18 @@ int run_stem7x7(const void* src, const void* wk, void* out, int64_t N, int64_t H
     cudaError_t e = cudaMemsetAsync(bn_sums, 0, 2 * (size_t)n_out * sizeof(double), st);
     if (e != cudaSuccess) { set_error("stem7x7: memset: %s", cudaGetErrorString(e)); return (int)e; }
   }
-#define STEM(BN) (bn_sums ? launch_stem<BN, true>(tx, tw, ty, g, bn_sums, st) : launch_stem<BN, false>(tx, tw, ty, g, nullptr, st))
-  if (n_out == 64) return STEM(64);
-  if (n_out == 128) return STEM(128);
-  return STEM(256);
-#undef STEM
+  if (!bn_sums) return n_out == 64 ? launch_stem<64, false>(tx, tw, ty, g, nullptr, st) : launch_stem<128, false>(tx, tw, ty, g, nullptr, st);
+  // fused statistics: one [2][n_out] partial per CTA, added into bn_sums in CTA order
+  const int nparts = num_sms();
+  double* parts = nullptr;
+  rc = scratch_alloc(&parts, (size_t)nparts * 2 * n_out * sizeof(double), st);
+  if (rc) return rc;
+  const cudaError_t e = cudaMemsetAsync(parts, 0, (size_t)nparts * 2 * n_out * sizeof(double), st);
+  if (e != cudaSuccess) { set_error("stem7x7: memset: %s", cudaGetErrorString(e)); scratch_free(parts, st); return (int)e; }
+  rc = n_out == 64 ? launch_stem<64, true>(tx, tw, ty, g, parts, st) : launch_stem<128, true>(tx, tw, ty, g, parts, st);
+  if (!rc) rc = run_sum_partials_f64(parts, 2 * n_out, bn_sums, 2 * n_out, nparts, st);
+  const int rf = scratch_free(parts, st);
+  return rc ? rc : rf;
 }
 
 bool stem7x7_wgrad_applicable(int dtype, int64_t N, int64_t H, int64_t W, int64_t Cs, int64_t Cin, int64_t Cout, int64_t R,
@@ -491,9 +434,16 @@ int run_stem7x7_wgrad(const void* x, const void* dy, float* dw, int64_t N, int64
   cudaError_t e = cudaFuncSetAttribute(stem7x7_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) { set_error("stem7x7_wgrad: cudaFuncSetAttribute(smem=%zu): %s", smem, cudaGetErrorString(e)); return (int)e; }
   const int grid = g.num_tiles < num_sms() ? g.num_tiles : num_sms();
-  stem7x7_wgrad_kernel<<<grid, 192, smem, st>>>(tx, tdy, g, dw);
-  SIMCLR_CHECK_LAUNCH();
-  return SIMCLR_OK;
+  const int64_t dw_elems = 49 * Cin * 64;
+  float* ws = nullptr;                                      // [grid][49 * Cin * 64] per-CTA partials
+  rc = scratch_alloc(&ws, (size_t)grid * dw_elems * sizeof(float), st);
+  if (rc) return rc;
+  stem7x7_wgrad_kernel<<<grid, 160, smem, st>>>(tx, tdy, g, ws);
+  e = cudaGetLastError();
+  if (e != cudaSuccess) { set_error("stem7x7_wgrad: launch: %s", cudaGetErrorString(e)); scratch_free(ws, st); return (int)e; }
+  rc = run_sum_partials(ws, dw_elems, dw, dw_elems, grid, st);
+  const int rf = scratch_free(ws, st);
+  return rc ? rc : rf;
 }
 
 }  // namespace tc

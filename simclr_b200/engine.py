@@ -163,7 +163,7 @@ class Engine:
 
     def __init__(self, device=None, precision=None, conv_engine=None, ctx=None):
         if not torch.cuda.is_available():
-            raise SimclrError('simclr_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback')
+            raise SimclrError('simclr_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback')
         lib.load()
         self.device = torch.device(device if device is not None else 'cuda:%d' % torch.cuda.current_device())
         precision = precision or FLAGS.b200_precision
@@ -224,7 +224,7 @@ class Engine:
         self._sums_cursor += n_al
         return t
 
-    # -- packed tcgen05 operands -------------------------------------------------
+    # -- packed tensor-core operands -------------------------------------------------
     def register_packed(self, op):
         self._pack_ops.append(op)
         self._pack_table = None

@@ -58,7 +58,7 @@ def define_flags():
     f.DEFINE_string('master', None, 'Address/name of the TensorFlow master to use (inert).')
     f.DEFINE_string('model_dir', None, 'Model directory for training.')
     f.DEFINE_string('data_dir', None, 'Directory where dataset is stored.')
-    f.DEFINE_bool('use_tpu', True, 'Whether to run on TPU (inert: this implementation runs on B200).')
+    f.DEFINE_bool('use_tpu', True, 'Whether to run on TPU (inert: this implementation runs on H100).')
     f.DEFINE_string('tpu_name', None, 'The Cloud TPU to use for training (inert).')
     f.DEFINE_string('tpu_zone', None, '[Optional] GCE zone of the Cloud TPU (inert).')
     f.DEFINE_string('gcp_project', None, '[Optional] Project name for the Cloud TPU (inert).')
@@ -87,10 +87,10 @@ def define_flags():
     f.DEFINE_boolean('use_blur', True, 'Whether or not to use Gaussian blur for augmentation during pretraining.')
     # ---- engine flags (not in the reference) ----
     f.DEFINE_enum('b200_precision', 'bf16', ['bf16', 'fp32'],
-                  'Activation/operand storage type of the conv stack: bf16 (tcgen05 kind::f16, '
+                  'Activation/operand storage type of the conv stack: bf16 (wgmma bf16, '
                   'fp32 accumulate) or fp32 (parity mode).')
     f.DEFINE_enum('b200_conv_engine', 'tc', ['tc', 'tc3', 'simt'],
-                  'tc: tcgen05/TMA implicit GEMM (default). tc3: three-way split-bf16 products on the tcgen05 engine '
+                  'tc: wgmma/TMA implicit GEMM (default). tc3: three-way split-bf16 products on the wgmma engine '
                   '(fp32 storage, fp32-accurate: the tensor-core verification mode). '
                   'simt: CUDA-core fp32 verification engine.')
     f.DEFINE_integer('b200_num_classes', 1000, 'Classes of the supervised head when no dataset is read.')

@@ -1,5 +1,5 @@
 """LARS optimizer of the reference (`tf2/lars_optimizer.py`) as a multi-tensor
-sm_100a update: two launches per step over device pointer tables, fixed
+sm_90a update: two launches per step over device pointer tables, fixed
 reduction order (all replicas apply bit-identical updates).
 """
 import re
@@ -40,7 +40,7 @@ class LARSOptimizer:
         if use_nesterov or not classic_momentum:
             raise NotImplementedError(
                 'only classic momentum without Nesterov (the branch build_optimizer reaches, '
-                'tf2/lars_optimizer.py:99-115) is implemented on the B200 path')
+                'tf2/lars_optimizer.py:99-115) is implemented on the GPU path')
 
     # -- name filters (tf2/lars_optimizer.py:139-157) ------------------------
     def _use_weight_decay(self, param_name):

@@ -1,5 +1,5 @@
 """Model, heads, LR schedule and optimizer factory of the reference
-(`tf2/model.py`) on the B200 engine.  Same class / function names, constructor
+(`tf2/model.py`) on the H100 engine.  Same class / function names, constructor
 arguments and error behaviour; variables are laid out in flat buffers and the
 backward pass is an explicit schedule (`Model.backward`).
 """

@@ -1,4 +1,4 @@
-"""Contrastive objective of the reference (`tf2/objective.py`) on the B200 kernels.
+"""Contrastive objective of the reference (`tf2/objective.py`) on the H100 kernels.
 
 `add_contrastive_loss(hidden, hidden_norm, temperature, strategy)` keeps the
 reference signature and returns `(loss, logits_ab, labels)`.  The returned loss

@@ -1,4 +1,4 @@
-"""`momentum` and `adam` of the reference's `build_optimizer` (tf2/model.py:31-34) on the B200 path:
+"""`momentum` and `adam` of the reference's `build_optimizer` (tf2/model.py:31-34) on the H100 path:
 `tf.keras.optimizers.SGD(learning_rate, FLAGS.momentum, nesterov=True)` and
 `tf.keras.optimizers.Adam(learning_rate)` as element-wise kernels over the flat parameter buffer
 (`csrc/optim.cu`).  Same host interface as `LARSOptimizer` (`apply_gradients`, `iterations`,

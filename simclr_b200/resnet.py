@@ -1,5 +1,5 @@
 """ResNet of the reference (`tf2/resnet.py`) with an explicit forward/backward
-schedule on the sm_100a kernels -- no framework autograd on the GPU path.
+schedule on the sm_90a kernels -- no framework autograd on the GPU path.
 
 Class names, constructor arguments and the `resnet()` factory mirror
 `tf2/resnet.py:31-78,160-208,314-526,529-747`.  Every layer object has
@@ -216,8 +216,8 @@ class BatchNormRelu:  # pylint: disable=missing-docstring
 
 
 class ConvOp:
-    """Implicit-GEMM convolution on the tcgen05 engine (or the CUDA-core
-    verification engine).  `kernel` is the fp32 HWIO master; the tcgen05 engine
+    """Implicit-GEMM convolution on the wgmma engine (or the CUDA-core
+    verification engine).  `kernel` is the fp32 HWIO master; the wgmma engine
     reads K-major packed copies refreshed from the master on every forward."""
 
     def __init__(self, kernel, R, S, cin, cout, stride, stored_cin=None, need_dgrad=True):
@@ -322,9 +322,9 @@ class ConvOp:
         st = stream_ptr()
         assert dy.dtype == x.dtype, (dy.dtype, x.dtype)
         tc = e.conv_engine == 'tc'
-        # fp32 storage (verification mode): the tcgen05 wgrad kernel is bf16-only (MN-major tf32 needs a
+        # fp32 storage (verification mode): the wgmma wgrad kernel is bf16-only (MN-major tf32 needs a
         # different swizzle atom), so the fp32 wgrad runs on the CUDA-core engine.
-        # The tcgen05 wgrad also needs 16-byte rows of dY (Cout % 8 == 0 in bf16): an odd-width supervised head
+        # The wgmma wgrad also needs 16-byte rows of dY (Cout % 8 == 0 in bf16): an odd-width supervised head
         # (e.g. 10 classes) takes the CUDA-core kernel for that one small GEMM.
         if tc and x.dtype == torch.bfloat16 and self.cout % 8 == 0:
             self._timed(e, 'wgrad', x.shape, lambda: lib.conv2d_wgrad_tc(
@@ -357,7 +357,7 @@ def _convop_backward_tc3(self, e, saved, dy, need_dx, dx_dtype):
         self._timed(e, 'wgrad', x.shape, lambda: lib.conv2d_wgrad_tc3(
             xs[0], xs[1], xs[2], ds[0], ds[1], ds[2], self.kernel.grad, N, H, W, Cs, self.cin, self.cout, self.R, self.S,
             self.stride, st))
-    else:       # odd-width supervised head: 16-byte rows of dY are a tcgen05 wgrad requirement
+    else:       # odd-width supervised head: 16-byte rows of dY are a wgmma wgrad requirement
         lib.conv2d_wgrad_simt(x, dy, self.kernel.grad, F32, N, H, W, Cs, self.cin, self.cout, self.R, self.S,
                               self.stride, st)
     if not (need_dx and self.need_dgrad):

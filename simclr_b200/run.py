@@ -1,5 +1,5 @@
 """Pretraining driver: the flag surface and `single_step` of the reference's
-`tf2/run.py` on the B200 engine.
+`tf2/run.py` on the H100 engine.
 
 `python -m simclr_b200.run --train_batch_size=512 ...` (under torchrun for more
 than one GPU: one process per GPU, NCCL over NVLink) trains on synthetic

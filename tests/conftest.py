@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (B200); run with -m gpu on the GPU box')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (H100); run with -m gpu on a GPU host')
     # The CPU oracle scales negatively past ~32 threads on the 128-core GPU hosts.
     import torch
     torch.set_num_threads(min(16, os.cpu_count() or 1))

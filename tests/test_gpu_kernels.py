@@ -1,4 +1,4 @@
-"""Parity of every C-ABI kernel (except the tcgen05 engine, see
+"""Parity of every C-ABI kernel (except the tensor-core engine, see
 test_gpu_tc.py) against the CPU oracle on seeded inputs.  Integer outputs are
 compared bit-exactly; floats within the tolerance written at each assert
 (north_star: 1e-3 relative fp32)."""

@@ -1,4 +1,4 @@
-"""The rest of the run.py mode matrix on the B200 path (SURVEY.md section 8, rows N2-N4): finetuning with frozen
+"""The rest of the run.py mode matrix on the H100 path (SURVEY.md section 8, rows N2-N4): finetuning with frozen
 block groups, inference-mode evaluation, the momentum / adam optimizers, checkpoints + resume, TensorBoard
 metrics -- each against the oracle's restatement of the same reference code."""
 import collections

@@ -1,4 +1,4 @@
-"""Parity of the BENCHMARKED precision: bf16 storage + tcgen05 conv engine.
+"""Parity of the BENCHMARKED precision: bf16 storage + wgmma conv engine.
 
 The reference computes the step in fp32 (tf2/run.py:557-622).  bf16 activation storage is not
 a 1e-3 approximation of that.  On ANY state of this network (ResNet + 3 BN'd head layers +
@@ -102,7 +102,7 @@ def test_bf16_tc_step_matches_bf16_storage_oracle(flags, depth, B, kind, warm):
 def test_bf16_tc_loss_curve_20_steps(flags):
     """north_star: "loss curve matching reference within tolerance" at the benchmarked precision.
     20 consecutive LARS steps of config 1 (ResNet-18, batch 32, 64x64; a fresh structured batch per
-    step, lr 0.2, weight decay 1e-4) on the bf16 tcgen05 path against the fp32 oracle trajectory
+    step, lr 0.2, weight decay 1e-4) on the bf16 wgmma path against the fp32 oracle trajectory
     (which the fp32 verification mode reproduces to 1e-3, test_gpu_step.py).  Training is chaotic:
     the yardstick for "within tolerance" is how far the bf16-STORAGE ORACLE's own trajectory drifts
     from the fp32 one over the same 20 steps."""
@@ -137,7 +137,7 @@ def test_bf16_tc_loss_curve_20_steps(flags):
 
 
 def test_num_classes_not_multiple_of_8(flags):
-    """CIFAR-10-style supervised head (num_classes=10): the tcgen05 wgrad needs 16-byte output rows,
+    """CIFAR-10-style supervised head (num_classes=10): the wgmma wgrad needs 16-byte output rows,
     so this layer takes the CUDA-core fallback instead of failing the first backward."""
     from simclr_b200 import engine, run, flags_def
     from oracle import model as OM, step as OS

@@ -2,7 +2,7 @@
 config 1 of BASELINE.json (ResNet-18, batch 32, 64x64, one replica).
 
 fp32 storage + CUDA-core conv engine is the 1e-3 parity mode (north_star
-tolerance); the bf16 tcgen05 path is checked against the same oracle with the
+tolerance); the bf16 wgmma path is checked against the same oracle with the
 looser tolerance bf16 activations allow.  Both the reference initialisation
 (zero last-BN gamma => exactly-zero in-block conv gradients, SURVEY Q3) and a
 "warm" state are covered.
@@ -128,9 +128,9 @@ def test_step_parity_fp32(flags, warm):
 @pytest.mark.parametrize('warm', [False, True])
 @pytest.mark.parametrize('precision,conv_engine,tol', [('bf16', 'tc', 0.5), ('fp32', 'tc', 0.15), ('bf16', 'simt', 0.5)])
 def test_step_tensor_core_path(flags, precision, conv_engine, tol, warm):
-    """Same step through the tcgen05 engine.  This batch-32 problem amplifies activation
+    """Same step through the wgmma engine.  This batch-32 problem amplifies activation
     rounding ~100x (fp32 path: 6e-6 observed = 100 x 2^-24; tf32 operands: 7e-2; bf16
-    storage: 2.5e-1, identical for the tcgen05 and the CUDA-core engines), so in these
+    storage: 2.5e-1, identical for the wgmma and the CUDA-core engines), so in these
     modes the step is only required to agree in loss (1%) and in gradient direction
     (relative error < tol); the kernels themselves are pinned tightly in test_gpu_tc.py."""
     from oracle import step as OS
@@ -231,7 +231,7 @@ def test_step_parity_r50_bottleneck(flags, warm):
 @pytest.mark.parametrize('depth', [18, 50])
 def test_step_parity_tc3(flags, depth):
     """The north_star tolerance ON THE TENSOR PIPE: fp32 storage, every conv / dense GEMM as three-way
-    split-bf16 products on the tcgen05 engine (`--b200_conv_engine=tc3`), whole step against the oracle at
+    split-bf16 products on the wgmma engine (`--b200_conv_engine=tc3`), whole step against the oracle at
     1e-3 -- ResNet-18 (the network of config 1) and plain ResNet-50 bottlenecks; same fixtures and bar as
     the fp32 CUDA-core verification mode."""
     passed = [_step_vs_oracle_1e3(flags, 'fp32', 'tc3', depth, 'lars', sd, 'R%d fp32/tc3' % depth) for sd in (0, 2, 4)]

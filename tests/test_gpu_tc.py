@@ -1,4 +1,4 @@
-"""Parity of the tcgen05 / TMA implicit-GEMM engine (fprop, dgrad, wgrad, dense)
+"""Parity of the wgmma / TMA implicit-GEMM engine (fprop, dgrad, wgrad, dense)
 against the oracle's convolution on the same (bf16-rounded) inputs.
 
 bf16 x bf16 products are exact in fp32, so with fp32 outputs the only
@@ -16,7 +16,7 @@ pytestmark = pytest.mark.gpu
 
 # N, H, W, Cin, Cs, Cout, k, stride
 CASES = [
-    (2, 16, 16, 64, 64, 256, 1, 1),      # plain GEMM: activations through TMA, BN=256
+    (2, 16, 16, 64, 64, 256, 1, 1),      # plain GEMM: activations through TMA, two 128-column tiles
     (3, 10, 10, 256, 256, 64, 1, 1),     # M=300 (ragged last tile), BN=64
     (2, 12, 12, 64, 64, 64, 3, 1),       # gathered 3x3
     (2, 8, 8, 128, 128, 128, 3, 1),      # BN=128, two K blocks per tap
@@ -45,7 +45,7 @@ CASES = [
     (2, 224, 224, 3, 4, 64, 7, 2),       # the benchmark shape: Q = 112 of 128 GEMM rows real
     (40, 16, 16, 3, 4, 64, 7, 2),        # 320 tiles: several per CTA, slab ring and both accumulators wrap
     (2, 64, 64, 3, 4, 128, 7, 2),        # width multiplier 2: two 64-column boxes per tile
-    (1, 48, 40, 3, 4, 256, 7, 2),        # width multiplier 4, rectangular
+    (1, 48, 40, 3, 4, 256, 7, 2),        # width multiplier 4, rectangular: beyond the stem kernel's 128 columns, generic path
 ]
 
 
@@ -120,6 +120,11 @@ def test_tc_wgrad_bf16(case):
     lib.conv2d_wgrad_tc(xs.cuda(), dy.cuda(), dw, 1, N, H, W, Cs, Cin, Cout, k, k, s, stream_ptr())
     torch.cuda.synchronize()
     assert rel_err(dw, wo.grad) < 2e-4
+    # split / per-CTA partials are added in a fixed order: the same inputs give the same bits
+    dw2 = torch.full_like(dw, float('nan'))
+    lib.conv2d_wgrad_tc(xs.cuda(), dy.cuda(), dw2, 1, N, H, W, Cs, Cin, Cout, k, k, s, stream_ptr())
+    torch.cuda.synchronize()
+    assert torch.equal(dw, dw2)
 
 
 @pytest.mark.parametrize('case', [CASES[0], CASES[2], CASES[4], CASES[7], CASES[9]])
@@ -141,7 +146,7 @@ def test_tc_tf32(case):
     torch.cuda.synchronize()
     assert rel_err(y, yo) < 3e-3
     assert rel_err(dx, xo.grad) < 3e-3
-    # wgrad on tf32 operands is not implemented on the tcgen05 engine: must fail loudly, not silently
+    # wgrad on tf32 operands is not implemented on the wgmma engine: must fail loudly, not silently
     from simclr_b200._lib import SimclrError
     dw = torch.empty((k, k, Cin, Cout), device='cuda')
     with pytest.raises(SimclrError):
@@ -152,7 +157,7 @@ def test_tc_tf32(case):
                                    (16, 28, 28, 256, 512, 1, 2), (8, 56, 56, 64, 256, 1, 1)])
 def test_tc_matches_simt_large(shape):
     """Size-independent check at BASELINE-sized layers (many tiles per CTA, tiles crossing image
-    rows and images): tcgen05 vs the CUDA-core engine on the same bf16 inputs."""
+    rows and images): wgmma vs the CUDA-core engine on the same bf16 inputs."""
     from simclr_b200._lib import lib, stream_ptr
     N, H, W, C, Co, k, s = shape
     Ho, Wo = (H - 1) // s + 1, (W - 1) // s + 1
@@ -188,7 +193,7 @@ def _split(t):
 
 @pytest.mark.parametrize('case', [CASES[i] for i in (0, 1, 2, 4, 5, 6, 8, 12, 13, 16)])
 def test_tc3_split_bf16_fp32_accuracy(case):
-    """tc3 (fp32 operands split into three bf16 terms, six tcgen05 GEMMs summed in fp32): fprop, dgrad and
+    """tc3 (fp32 operands split into three bf16 terms, six wgmma GEMMs summed in fp32): fprop, dgrad and
     wgrad against the fp64 oracle conv on UNROUNDED fp32 inputs at 5e-6 -- three orders below a single
     bf16 pass (4e-3), at the level of an fp32 CUDA-core conv."""
     from simclr_b200._lib import lib, stream_ptr
