@@ -380,6 +380,30 @@ SIMCLR_API int simclr_augment(const uint8_t* src, const int64_t* src_offset, con
                               int64_t n, int64_t height, int64_t width, int64_t out_pixel_stride,
                               int64_t out_channel_offset, void* stream);
 
+/* Baseline JPEG decode of a batch (the tf.io.decode_jpeg inside the reference's TFDS input pipeline; here
+ * bit-exact with Pillow / libjpeg-turbo's JDCT_ISLOW + fancy upsampling, oracle/jpeg.py), writing the packed
+ * uint8 HWC layout simclr_augment reads.  The host (simclr_b200/jpeg.py) parses and validates the headers;
+ * this call only decodes what it was given: SOF0/SOF1 8-bit, one interleaved scan, 1 or 3 components, luma
+ * sampling h, v in {1, 2}, 1x1 chroma.
+ *   images    [n][40] int64 descriptors: 0 output byte offset, 1 H, 2 W, 3 ncomp, 4 hmax, 5 vmax, 6 MCUs per row,
+ *             7 MCU rows, 8 first block of the image in the workspace, 9 its block count, then per component c
+ *             (three slots each): 10+c block offset (component 0 at 0), 13+c blocks per row, 16+c block rows,
+ *             19+c / 22+c sampling h / v (1 for a single component), 25+c byte offset in `tables` of the
+ *             quantisation table (64 uint16, natural order), 28+c / 31+c of the DC / AC Huffman table
+ *   segments  [nseg][8] int64: image, first byte, end byte (offsets into `data`: the entropy-coded bytes of
+ *             one image, or of one restart interval), first MCU, MCU count.  One thread decodes one segment.
+ *   tables    Huffman tables of 1424 bytes: uint16 look[512] ((length << 8) | symbol of every code of <= 9 bits
+ *             indexed by the next 9 bits, 0 when longer), int32 maxcode[18], int32 valoff[18], uint8 vals[256]
+ *   workspace >= total_blocks * 192 bytes (int16 coefficients, then uint8 component planes padded to whole
+ *             MCUs), 16-byte aligned; max_blocks / max_pixels: the largest per-image block / pixel counts
+ *   out       image i is H*W*3 bytes at out + images[i][0]
+ *   error     [n] bytes, set to 1 where the entropy data ran out or held an invalid code: that image's output
+ *             is garbage and must be decoded elsewhere.  Reads never leave [first byte, end byte) of a segment. */
+SIMCLR_API int simclr_jpeg_decode(const int64_t* images, int64_t n, const int64_t* segments, int64_t nseg,
+                                  const uint8_t* tables, const uint8_t* data, int64_t total_blocks,
+                                  int64_t max_blocks, int64_t max_pixels, void* workspace, size_t workspace_bytes,
+                                  uint8_t* out, uint8_t* error, void* stream);
+
 /* The other optimizers of build_optimizer (tf2/model.py:29-44), element-wise over flat buffers of n floats.
  * hyper_dev: device float[1] staged by the caller (stream-ordered): SGD {lr}; Adam
  * {lr * sqrt(1 - beta2^t) / (1 - beta1^t)} with t the 1-based step. */

@@ -102,9 +102,14 @@ class TFRecordBuilder:
 
     IMAGE_KEY, LABEL_KEY = 'image', 'label'
 
-    def __init__(self, data_dir, name=None, num_classes=None, decode_threads=None):
+    def __init__(self, data_dir, name=None, num_classes=None, decode_threads=None, decode=None):
+        """decode: 'host' (Pillow on `decode_threads` threads) or 'device' (`jpeg.decode_batch`: JPEGs the sm_90a
+        decoder supports on the GPU, bit-exact with 'host', the rest with Pillow); default --b200_jpeg_decode."""
         from . import tfrecord
         self._tf = tfrecord
+        self.decode = decode or FLAGS['b200_jpeg_decode'].value
+        if self.decode not in ('host', 'device'):
+            raise ValueError("decode must be 'host' or 'device', got %r" % (self.decode,))
         root = os.path.join(data_dir, name) if name and os.path.isdir(os.path.join(data_dir, name)) else data_dir
         files = collections.defaultdict(list)
         self.dir = None
@@ -195,6 +200,13 @@ class TFRecordBuilder:
         """Parallel decode (Pillow releases the GIL): the `num_parallel_calls=AUTOTUNE` of the reference's map."""
         return list(self._pool.map(lambda t: self.fetch(split, t), tokens))
 
+    def fetch_device(self, split, tokens, device):
+        """-> (jpeg.DecodeJob, labels): the batch's decode enqueued on the device (image sizes in `job.hw` at once,
+        pixels from `job.finish()`); images the device decoder does not take go to Pillow on this builder's pool."""
+        from . import jpeg
+        del split
+        return jpeg.start_decode([t[0] for t in tokens], device, self._pool), [t[1] for t in tokens]
+
 
 def get_preprocess_fn(is_training, is_pretrain):
     """Get function that accepts an image and returns a preprocessed image (tf2/data.py:101-115)."""
@@ -253,6 +265,8 @@ def build_input_fn(builder, global_batch_size, topology, is_training):
                 yield (make_batch or make)(e, idx)
 
         def make(e, idx):
+            if getattr(builder, 'decode', 'host') == 'device':
+                return make_packed(e, idx)
             fetched = (builder.fetch_many(split_name, idx) if hasattr(builder, 'fetch_many')
                        else [builder.fetch(split_name, t) for t in idx])
             images = [torch.from_numpy(im) for im, _ in fetched]
@@ -272,6 +286,31 @@ def build_input_fn(builder, global_batch_size, topology, is_training):
             else:
                 feats = data_util.preprocess_for_eval_batch(images, H, H, crop=test_crop)
             lab = torch.nn.functional.one_hot(labels, num_classes).float().to(e.device)
+            return feats, lab
+
+        def make_packed(e, idx):
+            """`make` with the decode on the device: the same draws, in the same order, from the header sizes while
+            the decode runs; the augmentation reads the decoder's packed output."""
+            job, labels = builder.fetch_device(split_name, idx, e.device)
+            hw = [(int(h), int(w)) for h, w in job.hw]
+            n = len(idx)
+            if is_training:
+                view_draws = []
+                for _ in range(2 if pretrain else 1):
+                    draws = [data_util.draw_train_augmentation(h, w, jitter, rng) for h, w in hw]
+                    if jitter <= 0:
+                        draws = [dict(d, color=dict(d['color'], apply_jitter=False, apply_gray=False)) for d in draws]
+                    view_draws.append(draws)
+            src, offs, src_hw = job.finish()
+            if pretrain:
+                feats = torch.empty((n, H, H, 6), dtype=torch.float32, device=e.device)
+                for v, draws in enumerate(view_draws):
+                    data_util.preprocess_for_train_packed(src, offs, job.hw, draws, H, H, out=feats, channel_offset=3 * v)
+            elif is_training:
+                feats = data_util.preprocess_for_train_packed(src, offs, job.hw, view_draws[0], H, H)
+            else:
+                feats = data_util.preprocess_for_eval_packed(src, offs, job.hw, H, H, crop=test_crop)
+            lab = torch.nn.functional.one_hot(torch.tensor(labels, dtype=torch.int64), num_classes).float().to(e.device)
             return feats, lab
 
         return batches()

@@ -68,12 +68,20 @@ def preprocess_for_train_batch(images, draws, height, width, out=None, channel_o
     into `out` [n,height,width,C] at `channel_offset` (two views -> [B,H,W,6], tf2/data.py:55-58)."""
     import numpy as np
     e = get_engine()
-    n = len(images)
     offs, hw, total = [], [], 0
     for im in images:
         assert im.dtype == torch.uint8 and im.dim() == 3 and im.shape[2] == 3
         offs.append(total); hw.append([im.shape[0], im.shape[1]]); total += im.numel()
     src = torch.cat([im.reshape(-1) for im in images]).to(e.device)
+    return _augment_packed(src, np.asarray(offs, dtype=np.int64), np.asarray(hw, dtype=np.int32), hw, draws, height,
+                           width, out, channel_offset)
+
+
+def _augment_packed(src, src_offset, src_hw, hw, draws, height, width, out, channel_offset):
+    """One `simclr_augment` launch over packed images; `hw`: the [n][2] image sizes on the host (box checks)."""
+    import numpy as np
+    e = get_engine()
+    n = len(draws)
     box = np.asarray([d['box'] for d in draws], dtype=np.int32)
     for (y, x, h, w), (Hs, Ws) in zip(box, hw):
         if not (0 <= y and 0 <= x and h > 0 and w > 0 and y + h <= Hs and x + w <= Ws):
@@ -85,13 +93,31 @@ def preprocess_for_train_batch(images, draws, height, width, out=None, channel_o
         code = sum(int(op) << (2 * t) for t, op in enumerate(c['perm']))
         col[i] = [1.0 if c['apply_jitter'] else 0.0, code, c['brightness'], c['contrast'], c['saturation'], c['hue'],
                   1.0 if c['apply_gray'] else 0.0, 0.0]
-    t = lambda a: torch.from_numpy(a).to(e.device)
+    t = lambda a: torch.as_tensor(a).to(e.device)
     if out is None:
         out = e.empty((n, height, width, 3), torch.float32)
     assert out.dtype == torch.float32 and out.is_contiguous() and out.shape[:3] == (n, height, width)
-    lib.augment(src, t(np.asarray(offs, dtype=np.int64)), t(np.asarray(hw, dtype=np.int32)), t(box), t(flip), t(col),
+    lib.augment(src, t(src_offset).to(torch.int64), t(src_hw).to(torch.int32), t(box), t(flip), t(col),
                 out, n, height, width, out.shape[3], channel_offset, stream_ptr())
     return out
+
+
+def preprocess_for_train_packed(src, src_offset, src_hw, draws, height, width, out=None, channel_offset=0):
+    """`preprocess_for_train_batch` over images already packed on the device, as `jpeg.decode_batch` returns them:
+    src uint8 HWC images back to back, src_offset int64 [n], src_hw int32 [n][2] (host or device tensors / arrays).
+    The same kernel launch and results as the list form."""
+    import numpy as np
+    hw = src_hw.cpu().numpy() if isinstance(src_hw, torch.Tensor) else np.asarray(src_hw)
+    assert src.dtype == torch.uint8 and len(hw) == len(draws) == len(src_offset)
+    return _augment_packed(src, src_offset, src_hw, hw.tolist(), draws, height, width, out, channel_offset)
+
+
+def preprocess_for_eval_packed(src, src_offset, src_hw, height, width, crop=True, out=None, channel_offset=0):
+    """`preprocess_for_eval_batch` over packed images (see `preprocess_for_train_packed`)."""
+    import numpy as np
+    hw = src_hw.cpu().numpy() if isinstance(src_hw, torch.Tensor) else np.asarray(src_hw)
+    draws = [dict(box=_eval_box(int(Hs), int(Ws), height, width, crop), flip=False, color=_NO_COLOR) for Hs, Ws in hw]
+    return preprocess_for_train_packed(src, src_offset, src_hw, draws, height, width, out=out, channel_offset=channel_offset)
 
 
 # ---------------------------------------------------------------------------
@@ -168,17 +194,17 @@ def preprocess_for_eval_batch(images, height, width, crop=True, out=None, channe
     """`preprocess_for_eval` (tf2/data_util.py:478-494) for a batch of uint8 images: central crop of
     CROP_PROPORTION, bicubic resize, clip -- the crop / resize / clip stages of the augmentation kernel with the
     flip and the colour ops switched off.  Without `crop` the images must already be height x width."""
-    draws = []
-    for im in images:
-        Hs, Ws = im.shape[0], im.shape[1]
-        if crop:
-            box = center_crop_box(Hs, Ws, height, width)
-        else:
-            if (Hs, Ws) != (height, width):
-                raise ValueError('preprocess_for_eval(crop=False) needs %dx%d images, got %dx%d' % (height, width, Hs, Ws))
-            box = (0, 0, Hs, Ws)
-        draws.append(dict(box=box, flip=False, color=_NO_COLOR))
+    draws = [dict(box=_eval_box(im.shape[0], im.shape[1], height, width, crop), flip=False, color=_NO_COLOR)
+             for im in images]
     return preprocess_for_train_batch(images, draws, height, width, out=out, channel_offset=channel_offset)
+
+
+def _eval_box(Hs, Ws, height, width, crop):
+    if crop:
+        return center_crop_box(Hs, Ws, height, width)
+    if (Hs, Ws) != (height, width):
+        raise ValueError('preprocess_for_eval(crop=False) needs %dx%d images, got %dx%d' % (height, width, Hs, Ws))
+    return (0, 0, Hs, Ws)
 
 
 def preprocess_image(image, height, width, is_training=False, color_jitter_strength=0., test_crop=True, draws=None):

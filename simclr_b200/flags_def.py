@@ -93,6 +93,9 @@ def define_flags():
                   'tc: wgmma/TMA implicit GEMM (default). tc3: three-way split-bf16 products on the wgmma engine '
                   '(fp32 storage, fp32-accurate: the tensor-core verification mode). '
                   'simt: CUDA-core fp32 verification engine.')
+    f.DEFINE_enum('b200_jpeg_decode', 'host', ['host', 'device'],
+                  'Where data.TFRecordBuilder decodes JPEGs: host (Pillow on a thread pool) or device (sm_90a '
+                  'kernels, bit-exact with Pillow; other formats and unsupported JPEGs stay on the host).')
     f.DEFINE_integer('b200_num_classes', 1000, 'Classes of the supervised head when no dataset is read.')
     f.DEFINE_integer('b200_num_examples', 1281167, 'Examples per epoch when no dataset is read.')
     f.DEFINE_integer('b200_num_eval_examples', 50000, 'Evaluation examples when no dataset is read.')
