@@ -97,6 +97,12 @@ SIMCLR_API int simclr_contrast_metrics(const float* logits_ab, int64_t B, int64_
 SIMCLR_API int simclr_softmax_xent(const float* logits, const float* labels, int64_t rows, int64_t label_rows,
                                    int64_t classes, float grad_scale, float* loss, float* dlogits,
                                    void* stream);
+/* Knowledge distillation (SimCLRv2, the distillation colab's add_kd_loss): student, teacher logits
+ * [rows][classes] fp32.  out [2 + rows]: out[0] = T^2 * mean_r CE(softmax(teacher/T), softmax(student/T)),
+ * out[1] = fraction of rows whose student argmax equals the teacher argmax (lowest index on ties),
+ * out[2..] per-row CE.  dstudent = (softmax(student/T) - softmax(teacher/T)) * grad_scale (nullable). */
+SIMCLR_API int simclr_distill_xent(const float* student, const float* teacher, int64_t rows, int64_t classes,
+                                   float temperature, float grad_scale, float* out, float* dstudent, void* stream);
 SIMCLR_API int simclr_bias_add(float* y, const float* bias, int64_t rows, int64_t C, void* stream);
 SIMCLR_API int simclr_bias_grad(const float* dy, float* dbias, int64_t rows, int64_t C, void* stream);
 /* y += a*x  (weight-decay gradient of the supervised head, tf2/model.py:47-60). */

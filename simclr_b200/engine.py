@@ -20,11 +20,13 @@ class Variable:
     """A trainable tensor (name follows the Keras naming the reference's LARS
     filters rely on, tf2/model.py:40-42) or a moving statistic."""
 
-    def __init__(self, name, shape, init, trainable=True):
+    def __init__(self, name, shape, init, trainable=True, constant=False):
         self.name = name
         self.shape = tuple(shape)
         self.init = init
         self.trainable = trainable
+        # a frozen distillation teacher's variable: loaded before the first forward and never written after it
+        self.constant = constant
         self.value = None      # fp32 view into the flat parameter buffer
         self.grad = None       # fp32 view into the flat gradient buffer
 
@@ -60,10 +62,12 @@ class VarStore:
         # False while the layers of a frozen part are built (`trainable=False` Keras layers of a finetuning
         # run, tf2/resnet.py:548-549,619-692): their variables join the non-trainable list
         self.default_trainable = True
+        # True for a frozen distillation teacher: every variable is a constant, so there is no gradient buffer
+        self.constant = False
 
     def add(self, name, shape, init, trainable=True):
-        trainable = trainable and self.default_trainable
-        v = Variable(name, shape, init, trainable)
+        trainable = trainable and self.default_trainable and not self.constant
+        v = Variable(name, shape, init, trainable, constant=self.constant)
         (self.trainable if trainable else self.moving).append(v)
         return v
 

@@ -99,6 +99,17 @@ def define_flags():
     f.DEFINE_integer('b200_num_classes', 1000, 'Classes of the supervised head when no dataset is read.')
     f.DEFINE_integer('b200_num_examples', 1281167, 'Examples per epoch when no dataset is read.')
     f.DEFINE_integer('b200_num_eval_examples', 50000, 'Evaluation examples when no dataset is read.')
+    # SimCLRv2 distillation (distill.py): a frozen teacher's temperature-softened predictions train the student
+    f.DEFINE_string('b200_distill_teacher', None,
+                    'Teacher weights for distillation: a ckpt-N.npz, a TensorFlow checkpoint prefix, or a directory '
+                    '(its latest checkpoint).  With --train_mode=finetune the training loss becomes distillation '
+                    '(labels are not used); not allowed with --train_mode=pretrain.')
+    f.DEFINE_float('b200_distill_temperature', 1.0, 'Distillation temperature T.')
+    f.DEFINE_integer('b200_teacher_resnet_depth', None, 'Teacher resnet_depth (None: the student\'s).')
+    f.DEFINE_integer('b200_teacher_width_multiplier', None, 'Teacher width_multiplier (None: the student\'s).')
+    f.DEFINE_float('b200_teacher_sk_ratio', None, 'Teacher sk_ratio (None: the student\'s).')
+    f.DEFINE_float('b200_teacher_se_ratio', None, 'Teacher se_ratio (None: the student\'s).')
+    f.DEFINE_integer('b200_teacher_ft_proj_selector', None, 'Teacher ft_proj_selector (None: the student\'s).')
 
 
 define_flags()

@@ -208,9 +208,12 @@ class SupervisedHead:
 class Model:
     """Resnet model with projection or supervised layer (tf2/model.py:228-280)."""
 
-    def __init__(self, num_classes, seed=0, **kwargs):
+    def __init__(self, num_classes, seed=0, constant=False, **kwargs):
+        """`constant=True` (a frozen distillation teacher): every variable is non-trainable and is never written
+        after the first forward, so the model has no gradient buffer and its packed weights are made once."""
         e = get_engine()
         self.vs = VarStore()
+        self.vs.constant = constant
         self.resnet_model = resnet.resnet(
             resnet_depth=FLAGS.resnet_depth, width_multiplier=FLAGS.width_multiplier,
             cifar_stem=FLAGS.image_size <= 32, vs=self.vs)

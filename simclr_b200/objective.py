@@ -34,6 +34,24 @@ def add_supervised_loss(labels, logits, grad_scale=None):
     return out[0], dlogits
 
 
+def add_distillation_loss(student_logits, teacher_logits, temperature, grad_scale=None):
+    """SimCLRv2 distillation (the distillation colab's `add_kd_loss`): T^2 * mean_r CE(softmax(teacher/T),
+    softmax(student/T)).  Returns (loss, agreement, dstudent): `agreement` is the fraction of rows whose student
+    argmax equals the teacher argmax; with `grad_scale`, dstudent = (softmax(s/T) - softmax(t/T)) * grad_scale
+    (the step passes T / (rows * replicas)), else None."""
+    e = get_engine()
+    assert student_logits.dtype == torch.float32 and teacher_logits.dtype == torch.float32
+    assert student_logits.shape == teacher_logits.shape and student_logits.dim() == 2, \
+        (tuple(student_logits.shape), tuple(teacher_logits.shape))
+    student_logits, teacher_logits = student_logits.contiguous(), teacher_logits.contiguous()
+    rows, classes = student_logits.shape
+    out = e.empty((2 + rows,), torch.float32)
+    dstudent = e.empty((rows, classes), torch.float32) if grad_scale is not None else None
+    lib.distill_xent(student_logits, teacher_logits, rows, classes, float(temperature),
+                     0.0 if grad_scale is None else float(grad_scale), out, dstudent, stream_ptr())
+    return out[0], out[1], dstudent
+
+
 class _Ctx:
     pass
 

@@ -239,8 +239,11 @@ class ConvOp:
         if self.wf is None or self.wf.dtype != e.act_dtype:
             self.wf = e.empty((self.cout, Kp))
             kd = self.R * self.S * self.cout
-            self.wd = e.empty((self.cin, (kd + kbe - 1) // kbe * kbe)) if self.need_dgrad else None
-            e.register_packed(self)
+            self.wd = e.empty((self.cin, (kd + kbe - 1) // kbe * kbe)) if self.need_dgrad and not self.kernel.constant else None
+            if not self.kernel.constant:
+                e.register_packed(self)
+        elif self.kernel.constant:
+            return                           # a frozen teacher's weights: packed once, on its first forward
         if e.pack_token is not None and self.packed_token is e.pack_token:
             return                           # refreshed by engine.pack_all() at the start of this forward
         lib.pack_conv_weight(self.kernel.value, self.wf, self.wd, e.code(e.act_dtype), self.R, self.S, self.cin,

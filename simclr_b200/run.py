@@ -27,9 +27,19 @@ from ._lib import lib, stream_ptr
 class Trainer:
     """Owns model + optimizer and runs `single_step` (tf2/run.py:557-622)."""
 
-    def __init__(self, num_classes=None, num_examples=None, seed=0, engine=None):
+    def __init__(self, num_classes=None, num_examples=None, seed=0, engine=None, teacher=None):
+        """`teacher` (a `distill.Teacher`, finetune mode only): the training loss becomes SimCLRv2 distillation on
+        the teacher's logits, and the student's class count is the teacher's."""
         self.engine = engine or engine_lib.get_engine()
         self.strategy = self.engine.ctx
+        self.teacher = teacher
+        if teacher is not None:
+            if FLAGS.train_mode != 'finetune':
+                raise ValueError('distillation needs train_mode=finetune (got %r)' % FLAGS.train_mode)
+            if num_classes is not None and num_classes != teacher.num_classes:
+                raise ValueError('the student has %d classes but the teacher %d: distilling across label spaces is '
+                                 'not supported' % (num_classes, teacher.num_classes))
+            num_classes = teacher.num_classes
         self.num_classes = num_classes or FLAGS.b200_num_classes
         self.num_examples = num_examples or FLAGS.b200_num_examples
         self.model = model_lib.Model(self.num_classes, seed=seed)
@@ -113,6 +123,10 @@ class Trainer:
     def _forward_backward_top(self, features, labels, split):
         e, model, R = self.engine, self.model, self.strategy.num_replicas_in_sync
         st = stream_ptr()
+        teacher_logits = None
+        if self.teacher is not None:
+            # the frozen teacher on the same features, inference mode (moving statistics, nothing saved)
+            teacher_logits = self.teacher(features)
         projection_head_outputs, supervised_head_outputs = model(features, training=True)
         B = features.shape[0]
         loss = None
@@ -125,7 +139,17 @@ class Trainer:
             d_proj = obj_lib.contrastive_backward(ctx, 1.0 / (B * R))
             self.metrics['contrast_loss'] = con_loss
             self.metrics['logits_con'] = logits_con
-        if supervised_head_outputs is not None:
+        if supervised_head_outputs is not None and teacher_logits is not None:
+            # SimCLRv2 distillation replaces the supervised loss; labels are not used (the data may have none)
+            T = float(FLAGS.b200_distill_temperature)
+            kd_loss, agreement, d_sup = obj_lib.add_distillation_loss(
+                supervised_head_outputs, teacher_logits, T, grad_scale=T / (supervised_head_outputs.shape[0] * R))
+            loss = kd_loss
+            self.metrics['distill_loss'] = kd_loss
+            self.metrics['distill_acc'] = agreement
+            self.metrics['teacher_logits'] = teacher_logits
+            self.metrics['supervised_logits'] = supervised_head_outputs
+        elif supervised_head_outputs is not None:
             # l = concat([l, l], 0) (tf2/run.py:600-602): row r uses labels[r % B]
             sup_loss, d_sup = obj_lib.add_supervised_loss(labels, supervised_head_outputs,
                                                           grad_scale=1.0 / (supervised_head_outputs.shape[0] * R))
@@ -323,11 +347,15 @@ def main(argv):
     checkpoints every `checkpoint_steps` (resume from the latest one in --model_dir, or weights from --checkpoint),
     train/* metrics + learning rate flushed to TensorBoard event files at the same cadence.  Reading a dataset
     (TFDS) and SavedModel export are not part of this path (SURVEY.md section 8: N1 / N2)."""
-    from . import metrics as metrics_lib, checkpoint as ckpt_lib
+    from . import metrics as metrics_lib, checkpoint as ckpt_lib, distill as distill_lib
     if len(argv) > 1:
         raise app.UsageError('Too many command-line arguments.')
+    distill = FLAGS.mode != 'eval' and distill_lib.distilling()
     rank = init_distributed()
     engine_lib.set_engine(engine_lib.Engine())
+    # --b200_distill_teacher: the frozen teacher is rebuilt and reloaded from the flag on every start (student
+    # checkpoints hold the student only); its head fixes the student's class count
+    teacher = distill_lib.Teacher(FLAGS.b200_distill_teacher) if distill else None
     # --data_dir: a prepared TFDS directory (TFRecord shards, data.TFRecordBuilder), or an .npz of decoded images
     # (data.ArrayBuilder.from_npz); without it: synthetic tensors of the input contract
     builder = None
@@ -340,9 +368,9 @@ def main(argv):
             builder = data_lib.TFRecordBuilder(FLAGS.data_dir, FLAGS.dataset)
         builder.download_and_prepare()
         trainer = Trainer(num_classes=builder.info.features['label'].num_classes,
-                          num_examples=builder.info.splits[FLAGS.train_split].num_examples)
+                          num_examples=builder.info.splits[FLAGS.train_split].num_examples, teacher=teacher)
     else:
-        trainer = Trainer()
+        trainer = Trainer(teacher=teacher)
     R = trainer.strategy.num_replicas_in_sync
     dev = trainer.engine.device
     num_train_examples, num_classes = trainer.num_examples, trainer.num_classes
@@ -384,7 +412,12 @@ def main(argv):
         contrast_acc_metric = metrics_lib.Mean('train/contrast_acc')
         contrast_entropy_metric = metrics_lib.Mean('train/contrast_entropy')
         all_metrics.extend([contrast_loss_metric, contrast_acc_metric, contrast_entropy_metric])
-    if not pretrain or FLAGS.lineareval_while_pretraining:
+    if distill:
+        distill_loss_metric = metrics_lib.Mean('train/distill_loss')
+        distill_acc_metric = metrics_lib.Mean('train/distill_acc')          # agreement with the teacher's argmax
+        supervised_acc_metric = metrics_lib.Mean('train/supervised_acc')    # against the dataset labels
+        all_metrics.extend([distill_loss_metric, distill_acc_metric, supervised_acc_metric])
+    elif not pretrain or FLAGS.lineareval_while_pretraining:
         supervised_loss_metric = metrics_lib.Mean('train/supervised_loss')
         supervised_acc_metric = metrics_lib.Mean('train/supervised_acc')
         all_metrics.extend([supervised_loss_metric, supervised_acc_metric])
@@ -410,7 +443,13 @@ def main(argv):
                 metrics_lib.update_pretrain_metrics_train(contrast_loss_metric, contrast_acc_metric, contrast_entropy_metric,
                                                           m['contrast_loss'], m['logits_con'], None,
                                                           trainer.strategy.replica_id)
-            if 'supervised_loss' in m:
+            if distill:
+                distill_loss_metric.update_state(m['distill_loss'])
+                distill_acc_metric.update_state(m['distill_acc'])
+                if labels is not None:
+                    lab = labels.argmax(1)
+                    supervised_acc_metric.update_state((lab == m['supervised_logits'].argmax(1)).float().mean())
+            elif 'supervised_loss' in m:
                 metrics_lib.update_finetune_metrics_train(supervised_loss_metric, supervised_acc_metric,
                                                           m['supervised_loss'], labels, m['supervised_logits'])
             cur_step = trainer.optimizer.iterations
