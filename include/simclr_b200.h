@@ -292,7 +292,11 @@ SIMCLR_API int simclr_conv2d_wgrad_tc(const void* x, const void* dy, float* dw, 
  * v2 = bf16(v - v0 - v1) (`simclr_split_bf16x3`; `simclr_pack_conv_weight_part` writes part 0 / 1 / 2
  * of the packed weights in the layouts of `simclr_pack_conv_weight`), and a product is taken as
  * a0*b0 + a0*b1 + a1*b0 + a1*b1 + a0*b2 + a2*b0: six exact-product / fp32-accumulate GEMMs summed in
- * fp32 (TMA reduce-add); the dropped terms are 2^-24 relative.  Outputs are fp32 and overwritten. */
+ * fp32 (TMA reduce-add); the dropped terms are 2^-24 relative.  Outputs are fp32 and overwritten.
+ * The split is exact (v0 + v1 + v2 == v) for |v| >= 2^-110 up to the largest finite bf16 (~3.39e38); below
+ * 2^-110 v2 is a bf16 subnormal (kept, not flushed) and the split is v to within 2^-134.  From 0x7F7F8000
+ * (~3.396e38, where bf16(v) rounds to inf) up, no split exists: the kernel writes v0 = +-inf, v1 = -+inf,
+ * v2 = NaN.  No activation, gradient or weight of a training step comes near that range. */
 SIMCLR_API int simclr_split_bf16x3(const float* x, void* v0, void* v1, void* v2, int64_t n, void* stream);
 SIMCLR_API int simclr_pack_conv_weight_part(const float* w_hwio, void* wf, void* wd, int part, int64_t R,
                                             int64_t S, int64_t Cin, int64_t Cs, int64_t Cout, int64_t Kp,

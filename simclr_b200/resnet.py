@@ -339,7 +339,9 @@ class ConvOp:
         if not (need_dx and self.need_dgrad):
             return None
         dx = e.empty((N, H, W, self.cin), dx_dtype or e.act_dtype)
-        if tc:
+        # the wgmma dgrad gathers 16-byte rows of dY as well: an odd-width head (e.g. 10 or 100 classes when
+        # finetuning) takes its dX from the CUDA-core kernel on the fp32 master
+        if tc and (self.cout * dy.element_size()) % 16 == 0:
             self._timed(e, 'dgrad', x.shape, lambda: lib.conv2d_dgrad_tc(
                 dy, self.wd, dx, e.code(dy.dtype), e.code(dx.dtype), N, H, W, self.cin, self.cout, self.R, self.S,
                 self.stride, st))
@@ -365,9 +367,11 @@ def _convop_backward_tc3(self, e, saved, dy, need_dx, dx_dtype):
                               self.stride, st)
     if not (need_dx and self.need_dgrad):
         return None
-    if ds is None:
-        ds = self._split(e, dy)
     dx = e.empty((N, H, W, self.cin), torch.float32)
+    if ds is None:  # the wgmma dgrad gathers 16-byte rows of dY too: the odd-width head's dX on the CUDA cores
+        lib.conv2d_dgrad_simt(dy, self.kernel.value, dx, F32, F32, N, H, W, self.cin, self.cout, self.R, self.S,
+                              self.stride, st)
+        return dx
     self._timed(e, 'dgrad', x.shape, lambda: lib.conv2d_dgrad_tc3(
         ds[0], ds[1], ds[2], self.wd3[0], self.wd3[1], self.wd3[2], dx, N, H, W, self.cin, self.cout, self.R, self.S,
         self.stride, st))
