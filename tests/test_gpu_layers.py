@@ -5,7 +5,10 @@ The inventory is taken from the model itself: one eager bf16 / `tc` step per ben
 (4 views), with `conv2d_{fprop,dgrad,wgrad}_tc` wrapped to record every launch.  Each distinct launch is then
 replayed as the step issues it (same dtypes, fused BatchNorm sums where the step fuses them, bf16 dX, fp32 dW)
 on seeded inputs, at the recorded batch and at a batch with more 128-row tiles than the GPU has SMs, into
-NaN-filled outputs, and compared per element with torch's own convolution in float64 on the GPU:
+NaN-filled outputs, and compared per element with torch's own convolution in float64 on the GPU.  Inside a step
+`Engine.begin_step` switches `set_accumulate_prezeroed(1)` on: every fused-sums fprop then adds into a slice of the
+zeroed sums pool and every wgrad into a slice of the zeroed flat gradient buffer.  Each launch is replayed in every
+mode the step ran it in, and a fused fprop or wgrad also with the mode off (the call zeroes its own output):
 
     |got - ref| <= rho * |ref| + tau * A
 
@@ -68,7 +71,8 @@ def _fmt(key):
 
 @pytest.fixture(scope='module')
 def inventory():
-    """{family: {launch key: N}}: every tensor-core conv launch of one eager bf16 / tc step per family."""
+    """{family: ({launch key: N}, {launch key: set of pre-zeroed modes})}: every tensor-core conv launch of one
+    eager bf16 / tc step per family."""
     from simclr_b200 import engine, run, flags_def
     from simclr_b200._lib import lib
     F = flags_def.FLAGS
@@ -86,28 +90,37 @@ def inventory():
             g = torch.Generator().manual_seed(3)
             f = torch.rand(B, S, S, 6, generator=g).cuda()
             lab = torch.nn.functional.one_hot(torch.randint(0, 1000, (B,), generator=g), 1000).float().cuda()
-            launches = {}
+            launches, modes = {}, {}
+            state = {'pz': 0}
             with pytest.MonkeyPatch.context() as mp:
+                setpz = getattr(lib, 'set_accumulate_prezeroed')
+
+                def wrap_pz(on, _fn=setpz):
+                    state['pz'] = int(on)
+                    return _fn(on)
+                mp.setattr(lib, 'set_accumulate_prezeroed', wrap_pz)
                 for name in KINDS:
                     fn = getattr(lib, name)             # _Lib.__getattr__ caches the bound call on the instance
 
                     def wrap(*a, _fn=fn, _name=name):
                         key, N = _launch_key(_name, a)
                         launches[key] = max(N, launches.get(key, 0))
+                        modes.setdefault(key, set()).add(state['pz'])
                         return _fn(*a)
                     mp.setattr(lib, name, wrap)
                 trainer.single_step(f, lab)
                 torch.cuda.synchronize()
-            inv[fam] = launches
+            inv[fam] = (launches, modes)
             del trainer
             torch.cuda.empty_cache()
     finally:
         for k, v in saved.items():
             setattr(F, k, v)
-    for fam, launches in inv.items():
+        lib.set_accumulate_prezeroed(0)
+    for fam, (launches, modes) in inv.items():
         print('\n%s: %d distinct tensor-core conv launches' % (fam, len(launches)))
         for key in sorted(launches, key=_fmt):
-            print('    N %3d  %s' % (launches[key], _fmt(key)))
+            print('    N %3d  %-70s prezeroed %s' % (launches[key], _fmt(key), sorted(modes[key])))
     return inv
 
 
@@ -153,12 +166,16 @@ LANDMARKS = {
 
 @pytest.mark.parametrize('family', list(FAMILIES))
 def test_inventory_landmarks(inventory, family):
-    launches = inventory[family]
+    launches, modes = inventory[family]
     missing = [what for what, kind, pred in LANDMARKS[family] if not _has(launches, kind, pred)]
     assert not missing, '%s no longer launches: %s' % (family, missing)
     # the bf16 step writes bf16 dX from every dgrad and fp32 dW from every wgrad
     assert all(k[10] == BF16 for k in launches if k[0] == 'dgrad'), family
     assert all(k[10] == F32 for k in launches if k[0] == 'wgrad'), family
+    # every wgrad adds into the step's zeroed flat gradient buffer and every fused fprop into its zeroed sums pool
+    acc = [k for k in launches if accumulates(k)]
+    assert any(k[0] == 'wgrad' for k in acc) and any(k[0] == 'fprop' for k in acc), family
+    assert all(modes[k] == {1} for k in acc), [(_fmt(k), modes[k]) for k in acc if modes[k] != {1}]
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -186,9 +203,27 @@ def _ref_dw(x, dy, k, s, w_shape):
     return torch.autograd.grad(conv_reference(x, w, k, s), w, dy)[0]
 
 
-def check_launch(key, N, seed=0):
+def accumulates(key):
+    """True for the launches whose output depends on the pre-zeroed mode: wgrads and fprops with fused sums."""
+    return key[0] == 'wgrad' or (key[0] == 'fprop' and key[11])
+
+
+GUARD = 64          # NaN elements on each side of a pre-zeroed output slice
+
+
+def _zeroed_slice(n, dtype):
+    """A zeroed slice of a NaN-filled buffer, as the step's pools hand out sums and dW; returns (slice, guards)."""
+    buf = torch.full((GUARD + n + GUARD,), float('nan'), dtype=dtype, device='cuda')
+    buf[GUARD:GUARD + n].zero_()
+    return buf[GUARD:GUARD + n], (buf[:GUARD], buf[GUARD + n:])
+
+
+def check_launch(key, N, seed=0, prezeroed=0):
     """Replays one launch at batch N into NaN-filled outputs.  Returns (worst bound ratio, location, sums
-    error) -- the sums error is max |S - sum| / allowance over channels, None without fused sums."""
+    error) -- the sums error is max |S - sum| / allowance over channels, None without fused sums.
+    prezeroed = 1 replays it as the step issues it: with set_accumulate_prezeroed(1), fused sums into a zeroed
+    slice of a NaN fp64 buffer and dW into a zeroed slice of a NaN flat buffer; an overwritten NaN guard of
+    either is an infinite ratio."""
     from simclr_b200._lib import lib, stream_ptr, DTYPE_CODE
     kind, H, W, Cs, Cin, Cout, R, S, s, din, dout, fused = key
     assert R == S and din == BF16, key
@@ -200,13 +235,22 @@ def check_launch(key, N, seed=0):
     xs = x if Cs == Cin else torch.cat([x, torch.zeros(N, H, W, Cs - Cin, dtype=BF16, device='cuda')], -1).contiguous()
     x64, w64, dy64 = x.double(), w.double(), dy.double()
     st = stream_ptr()
-    lib.set_accumulate_prezeroed(0)            # the calls zero their own accumulation outputs
+    # mode 0: the calls zero their own accumulation outputs
+    prev = lib.set_accumulate_prezeroed(prezeroed)
+    guards = ()
     sums_err = None
     if kind == 'fprop':
         wf, _ = _pack(w, BF16, R, Cin, Cs, Cout, want_wd=False)
         got = torch.full((N, Ho, Wo, Cout), float('nan'), dtype=dout, device='cuda')
-        sums = torch.full((2 * Cout,), float('nan'), dtype=torch.float64, device='cuda') if fused else None
-        lib.conv2d_fprop_tc(xs, wf, got, DTYPE_CODE[din], DTYPE_CODE[dout], N, H, W, Cs, Cout, R, S, s, sums, st)
+        sums = None
+        if fused and prezeroed:
+            sums, guards = _zeroed_slice(2 * Cout, torch.float64)
+        elif fused:
+            sums = torch.full((2 * Cout,), float('nan'), dtype=torch.float64, device='cuda')
+        try:
+            lib.conv2d_fprop_tc(xs, wf, got, DTYPE_CODE[din], DTYPE_CODE[dout], N, H, W, Cs, Cout, R, S, s, sums, st)
+        finally:
+            lib.set_accumulate_prezeroed(prev)
         ref = conv_reference(x64, w64, R, s)
         A = conv_reference(x64.abs(), w64.abs(), R, s)
         if fused:
@@ -218,16 +262,28 @@ def check_launch(key, N, seed=0):
     elif kind == 'dgrad':
         _, wd = _pack(w, BF16, R, Cin, Cs, Cout)
         got = torch.full((N, H, W, Cin), float('nan'), dtype=dout, device='cuda')
-        lib.conv2d_dgrad_tc(dy, wd, got, DTYPE_CODE[din], DTYPE_CODE[dout], N, H, W, Cin, Cout, R, S, s, st)
+        try:
+            lib.conv2d_dgrad_tc(dy, wd, got, DTYPE_CODE[din], DTYPE_CODE[dout], N, H, W, Cin, Cout, R, S, s, st)
+        finally:
+            lib.set_accumulate_prezeroed(prev)
         ref = _ref_dx(dy64, w64, R, s, (N, H, W, Cin))
         A = _ref_dx(dy64.abs(), w64.abs(), R, s, (N, H, W, Cin))
     else:
-        got = torch.full((R, S, Cin, Cout), float('nan'), dtype=dout, device='cuda')
-        lib.conv2d_wgrad_tc(xs, dy, got, DTYPE_CODE[din], N, H, W, Cs, Cin, Cout, R, S, s, st)
+        if prezeroed:
+            got, guards = _zeroed_slice(R * S * Cin * Cout, dout)
+            got = got.view(R, S, Cin, Cout)
+        else:
+            got = torch.full((R, S, Cin, Cout), float('nan'), dtype=dout, device='cuda')
+        try:
+            lib.conv2d_wgrad_tc(xs, dy, got, DTYPE_CODE[din], N, H, W, Cs, Cin, Cout, R, S, s, st)
+        finally:
+            lib.set_accumulate_prezeroed(prev)
         ref = _ref_dw(x64, dy64, R, s, (R, S, Cin, Cout))
         A = _ref_dw(x64.abs(), dy64.abs(), R, s, (R, S, Cin, Cout))
     torch.cuda.synchronize()
     ratio, where = _ratio(got, ref, A, RHO[dout], TAU)
+    if not all(bool(torch.isnan(gd).all()) for gd in guards):
+        ratio, where = math.inf, 'NaN guard around the pre-zeroed slice overwritten'
     return ratio, where, sums_err
 
 
@@ -242,17 +298,25 @@ def _large_n(key, N, sms):
     return n if n > N else None
 
 
+def replay_modes(key, recorded=(0,)):
+    """The pre-zeroed modes to replay a launch in: every mode it was recorded in, and mode 0 as well where the
+    mode changes what the call does (wgrad, fused fprop)."""
+    return sorted(set(recorded) | ({0} if accumulates(key) else set()))
+
+
 def _run_launches(items, what):
-    """items: [(key, N)].  Checks each, prints the worst ratio per launch and fails listing every offender."""
+    """items: [(key, N)] or [(key, N, prezeroed)].  Checks each, prints the worst ratio per launch and fails
+    listing every offender."""
     bad, worst = [], 0.0
     t0 = time.time()
-    for key, N in items:
-        ratio, where, sums_err = check_launch(key, N)
+    for item in items:
+        key, N, pz = item if len(item) == 3 else item + (0,)
+        ratio, where, sums_err = check_launch(key, N, prezeroed=pz)
         worst = max(worst, ratio)
-        print('    %-70s N %4d  worst |err|/bound %.3f at %s%s' % (
-            _fmt(key), N, ratio, where, '' if sums_err is None else '  sums %.3f' % sums_err))
+        print('    %-70s N %4d  pz %d  worst |err|/bound %.3f at %s%s' % (
+            _fmt(key), N, pz, ratio, where, '' if sums_err is None else '  sums %.3f' % sums_err))
         if not ratio <= 1.0 or (sums_err is not None and not sums_err <= 1.0):
-            bad.append((_fmt(key), N, ratio, where, sums_err))
+            bad.append((_fmt(key), N, 'prezeroed %d' % pz, ratio, where, sums_err))
     print('%s: %d launches, worst |err|/(rho|ref| + tau A) = %.3f (tau = 2^%.1f), %.1f s' % (
         what, len(items), worst, math.log2(TAU), time.time() - t0))
     assert not bad, bad
@@ -261,16 +325,17 @@ def _run_launches(items, what):
 @pytest.mark.parametrize('size', ['recorded', 'large'])
 @pytest.mark.parametrize('family', list(FAMILIES))
 def test_launches_vs_fp64(inventory, family, size):
-    """Each distinct conv launch of the family's bf16 step, per element against fp64."""
-    launches = inventory[family]
-    if size == 'recorded':
-        items = sorted(launches.items(), key=lambda kv: _fmt(kv[0]))
-    else:
+    """Each distinct conv launch of the family's bf16 step, per element against fp64, in every pre-zeroed mode
+    the step ran it in (and with the mode off)."""
+    launches, modes = inventory[family]
+    items = sorted(launches.items(), key=lambda kv: _fmt(kv[0]))
+    if size == 'large':
         sms = torch.cuda.get_device_properties(0).multi_processor_count
-        items = [(k, _large_n(k, n, sms)) for k, n in sorted(launches.items(), key=lambda kv: _fmt(kv[0]))]
+        items = [(k, _large_n(k, n, sms)) for k, n in items]
         items = [(k, n) for k, n in items if n is not None]
         assert items, 'the time budget leaves no launch at a larger batch'
-    _run_launches(items, '%s at the %s batch' % (family, size))
+    _run_launches([(k, n, pz) for k, n in items for pz in replay_modes(k, modes[k])],
+                  '%s at the %s batch' % (family, size))
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -324,7 +389,7 @@ EDGES = [
 
 @pytest.mark.parametrize('key,N', EDGES, ids=[_fmt(k).replace(' ', '') + '-N%d' % n for k, n in EDGES])
 def test_edge_launch_vs_fp64(key, N):
-    _run_launches([(key, N)], 'edge')
+    _run_launches([(key, N, pz) for pz in replay_modes(key, (1,))], 'edge')
 
 
 def test_strided_1x1_dgrad_zero_classes():
