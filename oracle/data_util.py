@@ -5,8 +5,6 @@ explicit argument here (`draws`), so the deterministic arithmetic can be
 compared with the CUDA kernels on identical draws.  TF op semantics follow
 SURVEY.md Appendix A9.
 """
-import math
-
 import torch
 import torch.nn.functional as F
 
@@ -113,7 +111,7 @@ def adjust_hue(image, delta):
 
 def to_grayscale(image):
     """tf2/data_util.py:46-50: rgb_to_grayscale weights, tiled to 3 channels."""
-    w = torch.tensor([0.2989, 0.5870, 0.1140], dtype=image.dtype)
+    w = torch.tensor([0.2989, 0.5870, 0.1140], dtype=image.dtype, device=image.device)
     g = (image * w).sum(-1, keepdim=True)
     return g.repeat(*([1] * (image.dim() - 1)), 3)
 
@@ -160,27 +158,43 @@ def _keys_cubic_table(a=-0.5, table_size=1024, dtype=torch.float64):
     return torch.stack([w0, w1, w2, w3], -1)
 
 
+def _bicubic_axis_taps(in_size, out_size):
+    """The 4 taps of every output index of one axis of TF's bicubic resize (SURVEY A9).
+
+    TF takes the sample position in fp32, each operation rounded on its own (x86 builds do not contract to FMA):
+    `CalculateResizeScale` and `HalfPixelScaler` in tensorflow/core/util/image_resizer_state.h give
+    scale = (float)in / (float)out and in_f = ((float)o + 0.5f) * scale - 0.5f; `GetWeightsAndIndices` in
+    tensorflow/core/kernels/image/resize_bicubic_op.cc takes in = floor(in_f), delta = in_f - in and the table entry
+    lrintf(delta * 1024).  The entry's weights are evaluated here in fp64; out-of-range taps get weight 0 (their index
+    is clamped into the axis) and the rest are renormalised unless their sum is below 1000 FLT_MIN, as in TF.
+
+    in_size: an integer or an integer array (broadcast over its leading dimensions).
+    Returns (idx int64 [..., out, 4], w float64 [..., out, 4])."""
+    import numpy as np
+    f32 = np.float32
+    n = np.asarray(in_size, dtype=np.int64)[..., None]
+    o = np.arange(out_size, dtype=f32)
+    scale = n.astype(f32) / f32(out_size)
+    src = (o + f32(0.5)) * scale - f32(0.5)
+    fl = np.floor(src)
+    off = np.rint((src - fl) * f32(1024)).astype(np.int64)           # rint: round half to even, as lrintf
+    w = _keys_cubic_table(dtype=torch.float64).numpy()[off]
+    idx = fl.astype(np.int64)[..., None] - 1 + np.arange(4)
+    n = n[..., None]
+    w = np.where((idx >= 0) & (idx < n), w, 0.0)
+    tot = w.sum(-1, keepdims=True)
+    big = np.abs(tot) >= 1000.0 * 1.17549435e-38                      # std::numeric_limits<float>::min()
+    w = np.where(big, w / np.where(big, tot, 1.0), w)
+    return np.clip(idx, 0, n - 1), w
+
+
 def _bicubic_axis_weights(in_size, out_size, dtype):
-    """Half-pixel-centre bicubic sampling weights as a dense [out,in] matrix;
-    out-of-range taps dropped and weights renormalised (SURVEY A9)."""
-    table = _keys_cubic_table(dtype=torch.float64)
-    scale = in_size / out_size
-    W = torch.zeros(out_size, in_size, dtype=torch.float64)
-    for o in range(out_size):
-        src = (o + 0.5) * scale - 0.5
-        fl = math.floor(src)
-        frac = src - fl
-        off = int(round(frac * 1024))
-        w = table[off]
-        tot = 0.0
-        for t in range(4):
-            idx = fl - 1 + t
-            if 0 <= idx < in_size:
-                W[o, idx] += w[t]
-                tot += float(w[t])
-        if abs(tot) >= 1000.0 * 1.17549435e-38:      # std::numeric_limits<float>::min(), as in TF's kernel
-            W[o] /= tot
-    return W.to(dtype)
+    """Half-pixel-centre bicubic sampling weights (`_bicubic_axis_taps`) as a dense [out,in] matrix."""
+    import numpy as np
+    idx, w = _bicubic_axis_taps(in_size, out_size)
+    W = np.zeros((out_size, in_size))
+    np.add.at(W, (np.arange(out_size)[:, None], idx), w)
+    return torch.from_numpy(W).to(dtype)
 
 
 def crop_and_resize_bicubic(image, box, height, width):
@@ -188,8 +202,8 @@ def crop_and_resize_bicubic(image, box, height, width):
     (tf2/data_util.py:289-295, 319-320).  box = (y, x, h, w) integers."""
     y, x, h, w = box
     crop = image[y:y + h, x:x + w, :]
-    Wy = _bicubic_axis_weights(h, height, image.dtype)
-    Wx = _bicubic_axis_weights(w, width, image.dtype)
+    Wy = _bicubic_axis_weights(h, height, image.dtype).to(image.device)
+    Wx = _bicubic_axis_weights(w, width, image.dtype).to(image.device)
     return torch.einsum('oh,hwc,pw->opc', Wy, crop, Wx)
 
 

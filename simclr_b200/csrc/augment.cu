@@ -1,6 +1,7 @@
 // Train-time augmentation on device (tf2/data_util.py:443-475): crop + bicubic
 // resize (tf.image.resize BICUBIC: half-pixel centres, Keys a=-0.5, 1024-entry
-// coefficient table, out-of-range taps dropped and weights renormalised), flip,
+// coefficient table indexed by lrintf(frac * 1024) of the fp32 sample position,
+// out-of-range taps dropped and weights renormalised), flip,
 // colour jitter in a drawn order with a clip after each op, grayscale, final clip.
 // All random draws are inputs.  One CTA per output image; every thread owns the
 // same output pixels in every pass, only the contrast mean needs a block reduction.
@@ -14,12 +15,15 @@ constexpr int AT = 512;
 __device__ __forceinline__ double keys_inner(double x) { return ((1.5 * x - 2.5) * x) * x + 1.0; }          // |x| <= 1, A=-0.5
 __device__ __forceinline__ double keys_outer(double x) { return ((-0.5 * x + 2.5) * x - 4.0) * x + 2.0; }   // 1 < |x| < 2
 
-// weights/indices of the 4 taps for output index o (TF GetWeightsAndIndices, half-pixel scaler)
+// weights/indices of the 4 taps for output index o (TF GetWeightsAndIndices, half-pixel scaler).  The sample
+// position, its floor and the table offset are TF's fp32 arithmetic, each operation rounded on its own (no FMA
+// contraction): scale = in/out, src = (o + 0.5) * scale - 0.5, offset = lrintf((src - floor(src)) * 1024).  In
+// fp64 the offset differs for large crops (first at crop side 898 for a 224 output).
 __device__ __forceinline__ void bicubic_taps(int o, int in_size, int out_size, int* idx, float* w) {
-  const double scale = (double)in_size / (double)out_size;
-  const double src = ((double)o + 0.5) * scale - 0.5;
-  const double fl = floor(src);
-  const int off = (int)lrint((src - fl) * 1024.0);
+  const float scale = __fdiv_rn((float)in_size, (float)out_size);
+  const float src = __fsub_rn(__fmul_rn(__fadd_rn((float)o, 0.5f), scale), 0.5f);
+  const float fl = floorf(src);
+  const int off = (int)lrintf(__fmul_rn(__fsub_rn(src, fl), 1024.f));
   const double x = (double)off / 1024.0;
   double ww[4] = {keys_outer(x + 1.0), keys_inner(x), keys_inner(1.0 - x), keys_outer(2.0 - x)};
   double tot = 0.0;
