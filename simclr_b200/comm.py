@@ -13,6 +13,7 @@ P2P, SIMCLR_COMM=nccl): the callers then use torch.distributed / NCCL for the sa
 collectives.  Either path computes the same values; the peer path is what the scaling
 numbers are measured with.
 """
+import collections
 import os
 
 import torch
@@ -26,37 +27,62 @@ SLOT_BYTES = 2 * MAX_CHANNELS * 8
 GATHER_CHANNELS = {'z': 4 << 20, 'lse': 256 << 10}     # bytes per rank
 
 
+Layout = collections.namedtuple('Layout', 'bn_off gather_off bn_flag_off gather_flag_off total')
+
+
+def layout(world):
+    """Byte offsets of the regions of one rank's allocation for `world` ranks (the same on every rank): the bn
+    slots, the gather region of each channel, the bn flag words, the flag words of each channel, and the total
+    size (a whole number of 4 KiB pages)."""
+    off = 0
+    bn_off = off; off += NSLOT * world * SLOT_BYTES
+    gather_off = {}
+    for name, cap in GATHER_CHANNELS.items():
+        gather_off[name] = off; off += world * cap
+    bn_flag_off = off; off += NSLOT * world * 8
+    gather_flag_off = {}
+    for name in GATHER_CHANNELS:
+        gather_flag_off[name] = off; off += world * 8
+    return Layout(bn_off, gather_off, bn_flag_off, gather_flag_off, (off + 4095) // 4096 * 4096)
+
+
+def gather_fits(channel, nbytes):
+    """Whether a tensor of `nbytes` per rank can go through the peer-memory gather `channel`; a larger one, or
+    one that is not a 16-byte multiple, is gathered through NCCL."""
+    return 0 < nbytes <= GATHER_CHANNELS[channel] and nbytes % 16 == 0
+
+
 class PeerComm:
-    def __init__(self, group, device):
-        import torch.distributed._symmetric_memory as symm
-        self.group = group if group is not None else dist.group.WORLD
-        self.world = dist.get_world_size(self.group)
-        self.rank = dist.get_rank(self.group)
-        self.device = device
+    def __init__(self, rank, world, buf, peers_dev, handle=None):
+        """`buf`: this rank's zeroed allocation of `layout(world).total` bytes; `peers_dev`: the address of a
+        device array of the `world` ranks' `buf` base pointers, in rank order.  `create` makes both in symmetric
+        memory (`handle` keeps that rendezvous alive)."""
+        self.rank, self.world = rank, world
+        self.buf, self.peers_dev, self.handle = buf, peers_dev, handle
+        self.device = buf.device
         self.slot_bytes = SLOT_BYTES
-        W = self.world
-        off = 0
-        self.bn_off = off; off += NSLOT * W * SLOT_BYTES
-        self.gather_off = {}
-        for name, cap in GATHER_CHANNELS.items():
-            self.gather_off[name] = off; off += W * cap
-        self.bn_flag_off = off; off += NSLOT * W * 8
-        self.gather_flag_off = {}
-        for name in GATHER_CHANNELS:
-            self.gather_flag_off[name] = off; off += W * 8
-        self.total = (off + 4095) // 4096 * 4096
-        self.buf = symm.empty(self.total, dtype=torch.uint8, device=device)
-        self.handle = symm.rendezvous(self.buf, self.group.group_name)
-        self.peers_dev = int(self.handle.buffer_ptrs_dev)
-        self.buf.zero_()
+        self.bn_off, self.gather_off, self.bn_flag_off, self.gather_flag_off, self.total = layout(world)
+        assert buf.numel() >= self.total, (buf.numel(), self.total)
+        device = self.device
         # sequence numbers (start at 1: flag words start at 0) and CTA arrival counters, local memory
         # [sequence, nanoseconds spent waiting for peers] per channel
         self.bn_seq = torch.tensor([1, 0], dtype=torch.int64, device=device)
         self.gather_seq = {n: torch.tensor([1, 0], dtype=torch.int64, device=device) for n in GATHER_CHANNELS}
         self.gather_arrive = {n: torch.zeros(1, dtype=torch.int32, device=device) for n in GATHER_CHANNELS}
+
+    @staticmethod
+    def _symmetric(group, device):
+        import torch.distributed._symmetric_memory as symm
+        group = group if group is not None else dist.group.WORLD
+        world = dist.get_world_size(group)
+        buf = symm.empty(layout(world).total, dtype=torch.uint8, device=device)
+        handle = symm.rendezvous(buf, group.group_name)
+        buf.zero_()
+        comm = PeerComm(dist.get_rank(group), world, buf, int(handle.buffer_ptrs_dev), handle)
         torch.cuda.synchronize(device)
-        dist.barrier(self.group)             # nobody pushes before every buffer is zeroed
+        dist.barrier(group)             # nobody pushes before every buffer is zeroed
         torch.cuda.synchronize(device)
+        return comm
 
     @staticmethod
     def create(group=None, device=None):
@@ -66,7 +92,7 @@ class PeerComm:
             return None
         device = device or torch.device('cuda', torch.cuda.current_device())
         try:
-            return PeerComm(group, device)
+            return PeerComm._symmetric(group, device)
         except Exception as exc:      # no P2P / symmetric memory on this system: NCCL carries the collectives
             if os.environ.get('SIMCLR_COMM') == 'peer_required':
                 raise
@@ -96,7 +122,7 @@ class PeerComm:
         """[...] -> [world, ...] (rank-major), a view of the local gather region of `channel`."""
         t = t.contiguous()
         nbytes = t.numel() * t.element_size()
-        if nbytes % 16 or nbytes > GATHER_CHANNELS[channel]:
+        if not gather_fits(channel, nbytes):
             raise ValueError('all_gather(%s): %d bytes per rank (need a 16-byte multiple <= %d)'
                              % (channel, nbytes, GATHER_CHANNELS[channel]))
         off = self.gather_off[channel]

@@ -280,17 +280,7 @@ __global__ void bn_finalize_kernel(const double* __restrict__ sums, double count
                                    int C) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-  const double m = sums[c] / count;
-  double var = sums[C + c] / count - m * m;      // biased variance (SyncBN form, A4)
-  if (var < 0.0) var = 0.0;
-  const float mf = (float)m, vf = (float)var;
-  const float r = rsqrtf(vf + eps);
-  const float g = gamma ? gamma[c] : 1.f;
-  const float b = beta ? beta[c] : 0.f;
-  const float sc = g * r;
-  mean[c] = mf; rstd[c] = r; scale[c] = sc; shift[c] = b - mf * sc;
-  if (mm) mm[c] = mm[c] - (mm[c] - mf) * (1.f - momentum);
-  if (mv) mv[c] = mv[c] - (mv[c] - vf) * (1.f - momentum);
+  bn_finalize_channel(sums[c], sums[C + c], count, gamma, beta, eps, momentum, mm, mv, mean, rstd, scale, shift, c);
 }
 
 // The host sizes the grid so that gridDim*BT*8 is a multiple of C whenever it can: a thread then

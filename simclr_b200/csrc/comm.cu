@@ -97,17 +97,7 @@ bn_finalize_sync_kernel(Peers P, const double* __restrict__ sums, double count_l
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     double s0 = 0.0, s1 = 0.0;
     for (int r = 0; r < P.world; ++r) { s0 += __ldcg(all + r * slot_doubles + c); s1 += __ldcg(all + r * slot_doubles + C + c); }
-    const double m = s0 / count;
-    double var = s1 / count - m * m;            // biased variance (SyncBN form, SURVEY A4)
-    if (var < 0.0) var = 0.0;
-    const float mf = (float)m, vf = (float)var;
-    const float r_ = rsqrtf(vf + eps);
-    const float g = gamma ? gamma[c] : 1.f;
-    const float b = beta ? beta[c] : 0.f;
-    const float sc = g * r_;
-    mean[c] = mf; rstd[c] = r_; scale[c] = sc; shift[c] = b - mf * sc;
-    if (mm) mm[c] = mm[c] - (mm[c] - mf) * (1.f - momentum);
-    if (mv) mv[c] = mv[c] - (mv[c] - vf) * (1.f - momentum);
+    bn_finalize_channel(s0, s1, count, gamma, beta, eps, momentum, mm, mv, mean, rstd, scale, shift, c);
   }
   __syncthreads();
   if (threadIdx.x == 0) *seq_dev = seq + 1;

@@ -99,6 +99,27 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// BatchNorm finalize of channel c from the (global) sums s0 = sum x, s1 = sum x^2 over `count` rows: mean, rstd,
+// scale, shift and the moving-average update.  bn_finalize_kernel (bn.cu) and the SyncBN exchange (comm.cu) both
+// call it, so the peer-memory and NCCL paths of a multi-GPU step give the same bits.  The fused operations are
+// spelled out: left to the compiler, E[x^2] - mean^2 was contracted in one kernel and not in the other.
+__device__ __forceinline__ void bn_finalize_channel(double s0, double s1, double count, const float* gamma,
+                                                    const float* beta, float eps, float momentum, float* mm, float* mv,
+                                                    float* mean, float* rstd, float* scale, float* shift, int c) {
+  const double m = s0 / count;
+  double var = fma(-m, m, s1 / count);          // biased variance (SyncBN form, SURVEY A4)
+  if (var < 0.0) var = 0.0;
+  const float mf = (float)m, vf = (float)var;
+  const float r = rsqrtf(vf + eps);
+  const float g = gamma ? gamma[c] : 1.f;
+  const float b = beta ? beta[c] : 0.f;
+  const float sc = __fmul_rn(g, r);
+  const float om = 1.f - momentum;
+  mean[c] = mf; rstd[c] = r; scale[c] = sc; shift[c] = fmaf(-mf, sc, b);
+  if (mm) mm[c] = fmaf(-(mm[c] - mf), om, mm[c]);
+  if (mv) mv[c] = fmaf(-(mv[c] - vf), om, mv[c]);
+}
+
 template <typename T> __device__ __forceinline__ float to_f(T v);
 template <> __device__ __forceinline__ float to_f<float>(float v) { return v; }
 template <> __device__ __forceinline__ float to_f<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }

@@ -11,6 +11,7 @@ import torch
 import torch.distributed as dist
 
 from ._lib import lib, DTYPE_CODE, F32, BF16, SimclrError, stream_ptr
+from .comm import gather_fits
 from .flags_def import FLAGS
 
 BATCH_NORM_EPSILON = 1e-5  # tf2/resnet.py:28
@@ -150,11 +151,12 @@ class ReplicaContext:
 
     def all_gather(self, t, channel=None):
         """[...] -> [R, ...] (rank-major).  `channel`: name of a peer-memory gather region ('z',
-        'lse'); without one (or without peer memory) the gather goes through NCCL."""
+        'lse'); without one, without peer memory, or when the tensor does not fit the channel (an odd
+        per-replica batch makes the lse no 16-byte multiple) the gather goes through NCCL."""
         R = self.num_replicas_in_sync
         if R == 1:
             return t.unsqueeze(0)
-        if self.comm is not None and channel is not None:
+        if self.comm is not None and channel is not None and gather_fits(channel, t.numel() * t.element_size()):
             return self.comm.all_gather(t, channel)
         t = t.contiguous()
         out = torch.empty((R * t.shape[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=t.device)

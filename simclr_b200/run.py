@@ -22,6 +22,7 @@ from . import engine as engine_lib
 from . import model as model_lib
 from . import objective as obj_lib
 from ._lib import lib, stream_ptr
+from .comm import gather_fits
 
 
 class Trainer:
@@ -206,6 +207,10 @@ class Trainer:
         warm-up and puts it back after the capture, so the first `replay()` is step
         `optimizer.iterations` of the schedule on the pre-capture weights.  The capture
         itself executes nothing and does not advance the schedule."""
+        R = self.strategy.num_replicas_in_sync
+        if R > 1 and not self.peer_collectives_fit(features):
+            raise RuntimeError('CUDA-graph capture with %d replicas needs the peer-memory collectives '
+                               '(strategy.comm); run eagerly instead' % R)
         self._static = (features, labels)
         opt, vs = self.optimizer, self.model.vs
         opt.ensure_built(self.model.trainable_variables)      # H2D table copies must not land in the capture
@@ -220,7 +225,6 @@ class Trainer:
         torch.cuda.current_stream().wait_stream(s)
         torch.cuda.synchronize()
         self.optimizer.stage_learning_rate()
-        R = self.strategy.num_replicas_in_sync
         if R == 1:
             self._graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self._graph):
@@ -229,9 +233,6 @@ class Trainer:
         else:
             # More than one replica: the in-step collectives are peer-memory kernels (capturable); the
             # gradient all-reduce is NCCL and stays between two graphs.
-            if self.strategy.comm is None:
-                raise RuntimeError('CUDA-graph capture with %d replicas needs the peer-memory collectives '
-                                   '(strategy.comm); run eagerly instead' % R)
             self._graph = torch.cuda.CUDAGraph()
             self._graph_bottom = None
             if self._overlap_ok():
@@ -252,6 +253,19 @@ class Trainer:
             vs.flat_value.copy_(snap[0]); vs.flat_moving.copy_(snap[1]); opt._flat_v.copy_(snap[2])
             opt.iterations = snap[3]
         return self._graph
+
+    def peer_collectives_fit(self, features):
+        """Whether every in-step collective of a step on `features` runs on the peer-memory kernels, as a CUDA
+        graph at more than one replica needs: peer memory is set up, and the NT-Xent all-gathers fit their
+        channels (an odd per-replica batch, or more than 4 MiB of embeddings per rank, goes through NCCL)."""
+        if self.strategy.comm is None:
+            return False
+        if FLAGS.train_mode != 'pretrain':
+            return True
+        head = self.model._projection_head.linear_layers
+        D = head[-1].num_classes if head else self.model.resnet_model.cout
+        rows = features.shape[0] * (features.shape[3] // 3)
+        return gather_fits('z', rows * D * 4) and gather_fits('lse', rows * 4)
 
     def replay(self):
         self.optimizer.prepare_replay()

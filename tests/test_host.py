@@ -141,6 +141,38 @@ def _worker(rank, world, port, out):
     out.put((rank, 'ok'))
 
 
+def test_peer_comm_layout():
+    """comm.layout at W = 2..64: the bn slots, gather regions and flag words are disjoint and inside `total`; data
+    regions start on 16-byte boundaries (the kernels copy 16-byte vectors) and flag words on 8-byte ones."""
+    from simclr_b200 import comm
+    for W in range(2, 65):
+        L = comm.layout(W)
+        regions = [('bn %d/%d' % (k, q), L.bn_off + (k * W + q) * comm.SLOT_BYTES, comm.SLOT_BYTES, 16)
+                   for k in range(comm.NSLOT) for q in range(W)]
+        regions += [('flag bn %d/%d' % (k, q), L.bn_flag_off + (k * W + q) * 8, 8, 8)
+                    for k in range(comm.NSLOT) for q in range(W)]
+        for ch, cap in comm.GATHER_CHANNELS.items():
+            regions += [('%s %d' % (ch, q), L.gather_off[ch] + q * cap, cap, 16) for q in range(W)]
+            regions += [('flag %s %d' % (ch, q), L.gather_flag_off[ch] + q * 8, 8, 8) for q in range(W)]
+        regions.sort(key=lambda t: t[1])
+        assert regions[0][1] >= 0 and regions[-1][1] + regions[-1][2] <= L.total, W
+        assert L.total % 4096 == 0, W
+        for (n0, o0, s0, _), (n1, o1, _, _) in zip(regions, regions[1:]):
+            assert o0 + s0 <= o1, (W, n0, n1)
+        for name, off, _, align in regions:
+            assert off % align == 0, (W, name)
+
+
+def test_gather_fit_rule():
+    """The peer channels carry 16-byte multiples up to their capacity; the rest goes through NCCL (an odd
+    per-replica batch makes the [2B] fp32 lse 8B bytes)."""
+    from simclr_b200 import comm
+    assert comm.gather_fits('lse', 2 * 16 * 4) and not comm.gather_fits('lse', 2 * 3 * 4)
+    assert not comm.gather_fits('lse', 2 * 25 * 4) and comm.gather_fits('lse', 256 << 10)
+    assert comm.gather_fits('z', 2 * 4096 * 128 * 4) and not comm.gather_fits('z', 2 * 4097 * 128 * 4)
+    assert not comm.gather_fits('z', 0) and not comm.gather_fits('z', 8)
+
+
 def test_replica_context_gloo_world2():
     import torch.multiprocessing as mp
     ctx = mp.get_context('spawn')
