@@ -87,6 +87,67 @@ SIMCLR_API int simclr_contrast_metrics(const float* logits_ab, int64_t B, int64_
                                        float* out, void* stream);
 
 /* ------------------------------------------------------------------------- *
+ * Generalized contrastive loss (Chen, Luo, Li 2021; the intriguing-properties
+ * colab's generalized_contrastive_loss): L = loss_scaling * (L_align + lambda * L_dist)
+ * on z = l2_normalize(hidden) (simclr_ntxent_normalize), h1 = z[:B], h2 = z[B:].
+ * Global rows c in [0, 2G), G = R*B, are view-major over the job: c = v*G + r*B + i,
+ * read from z_all [R][2][B][D].  D <= 256 and, for the sliced Wasserstein terms,
+ * 2G <= 16384; larger shapes return SIMCLR_ERR_UNSUPPORTED.
+ * loss [3]: loss[0] = L, loss[1] = L_align, loss[2] = L_dist.
+ * ------------------------------------------------------------------------- */
+
+/* One workspace for every gcl entry below (the partial sums of the logsumexp term,
+ * the projections of the sliced Wasserstein term, the fp64 QR scratch). */
+SIMCLR_API size_t simclr_gcl_workspace_bytes(int64_t B, int64_t R, int64_t D);
+
+/* Philox-4x32-10 draws keyed by (seed, *step) (step: a device int64, so a replayed
+ * graph draws anew): prior [rows][D] N(0,1) (dist 0) or U(-1,1) (dist 1), rows
+ * l2-normalised if hidden_norm; wnormal [D][D] N(0,1).  Either, not both, may be
+ * NULL; one kernel launch. */
+SIMCLR_API int simclr_gcl_draw(int64_t seed, const int64_t* step, int64_t rows, int64_t D, int dist,
+                               int hidden_norm, float* prior, float* wnormal, void* stream);
+/* W [D][D] = Q of the QR of `normal` with Q's columns times sign(diag R) (Keras
+ * Orthogonal()): one-CTA Householder QR in fp64. */
+SIMCLR_API int simclr_gcl_orthogonal(const float* normal, int64_t D, float* W, void* workspace,
+                                     size_t workspace_bytes, void* stream);
+/* Local z [2][B][D]: loss[1] = sum (h1 - h2)^2 / (2 B D), dz = dL_align/dz (nullable);
+ * reads loss[2] (written by the dist forward) and writes loss[0]. */
+SIMCLR_API int simclr_gcl_align(const float* z, int64_t B, int64_t D, float lambda_weight, float loss_scaling,
+                                float* loss, float* dz, void* stream);
+/* Decoupled NT-Xent: lse [2][B] of the local rows against all 2G rows (self and
+ * positive included, no mask); loss[2] = mean(lse) - ln D. */
+SIMCLR_API int simclr_gcl_lse_forward(const float* z_all, int64_t B, int64_t R, int64_t D, int64_t replica_id,
+                                      float temperature, float* lse, float* loss, void* workspace,
+                                      size_t workspace_bytes, void* stream);
+/* dz [2][B][D] = d(sum over all 2G rows of lse)/d(local z): row- and column-side
+ * terms; lse_all is the all-gather of lse, layout [R][2][B]. */
+SIMCLR_API int simclr_gcl_lse_backward(const float* z_all, const float* lse_all, int64_t B, int64_t R, int64_t D,
+                                       int64_t replica_id, float temperature, float* dz, void* workspace,
+                                       size_t workspace_bytes, void* stream);
+/* Stable ascending sort of each of the `cols` columns of x_t [cols][n] (ties by
+ * row; -0 sorts as +0): sorted [cols][n] and perm [cols][n] (source rows), each
+ * nullable.  n <= 16384. */
+SIMCLR_API int simclr_gcl_sort(const float* x_t, int64_t n, int64_t cols, float* sorted, int32_t* perm,
+                               void* stream);
+/* Sliced Wasserstein distance of all 2G rows of z_all to the prior [2G][D] along
+ * the columns of W [D][D]: loss[2] = mean over 2G x D of (sort(prior W) - sort(z W))^2.
+ * Keeps perm [D][2G] (source row of each sorted position of z W) and
+ * diff [D][2G] = sort(z W) - sort(prior W) for the backward. */
+SIMCLR_API int simclr_gcl_swd_forward(const float* z_all, const float* prior, const float* W, int64_t B,
+                                      int64_t R, int64_t D, float* loss, int32_t* perm, float* diff,
+                                      void* workspace, size_t workspace_bytes, void* stream);
+/* dz [2][B][D] = dL_swd/d(local z): scatter 2 diff / (2G D) through perm, times W^T. */
+SIMCLR_API int simclr_gcl_swd_backward(const int32_t* perm, const float* diff, const float* W, int64_t B,
+                                       int64_t R, int64_t D, int64_t replica_id, float* dz, void* workspace,
+                                       size_t workspace_bytes, void* stream);
+/* dhidden = l2-normalise backward (identity without hidden_norm) of
+ * align_scale * dz_align + lse_scale * dz_lse + swd_scale * dz_swd (each nullable). */
+SIMCLR_API int simclr_gcl_normalize_backward(const float* z, const float* inv_norm, int hidden_norm, int64_t rows,
+                                             int64_t D, const float* dz_align, float align_scale,
+                                             const float* dz_lse, float lse_scale, const float* dz_swd,
+                                             float swd_scale, float* dhidden, void* stream);
+
+/* ------------------------------------------------------------------------- *
  * Supervised head loss  (tf2/objective.py:27-32) and small dense helpers
  * ------------------------------------------------------------------------- */
 

@@ -71,7 +71,8 @@ def _conv(v, ct):
 _LAUNCHES = {'ntxent_forward': 3, 'ntxent_backward': 2, 'contrast_metrics': 3, 'softmax_xent': 2, 'l2_loss': 2,
              'lars_apply': 2, 'bn_bwd_apply': 2, 'version': 0, 'last_error': 0, 'ntxent_workspace_bytes': 0,
              'set_accumulate_prezeroed': 0, 'memset_zero': 0, 'conv2d_fprop_tc3': 6, 'conv2d_dgrad_tc3': 6, 'conv2d_wgrad_tc3': 6,
-             'jpeg_decode': 3, 'distill_xent': 3}
+             'jpeg_decode': 3, 'distill_xent': 3, 'gcl_workspace_bytes': 0, 'gcl_lse_forward': 3,
+             'gcl_lse_backward': 2, 'gcl_swd_forward': 5, 'gcl_swd_backward': 2}
 
 
 class _Lib:

@@ -110,6 +110,14 @@ def define_flags():
     f.DEFINE_float('b200_teacher_sk_ratio', None, 'Teacher sk_ratio (None: the student\'s).')
     f.DEFINE_float('b200_teacher_se_ratio', None, 'Teacher se_ratio (None: the student\'s).')
     f.DEFINE_integer('b200_teacher_ft_proj_selector', None, 'Teacher ft_proj_selector (None: the student\'s).')
+    # Generalized contrastive loss (Chen, Luo, Li 2021; objective.generalized_contrastive_forward)
+    f.DEFINE_enum('b200_gcl_dist', 'none', ['none', 'logsumexp', 'normal', 'uniform'],
+                  'Pretraining objective: none is NT-Xent; otherwise the generalized contrastive loss with this '
+                  'distribution term: logsumexp (decoupled NT-Xent), or the sliced Wasserstein distance to a normal '
+                  'or uniform prior.  It uses --temperature (the colab\'s default is 1.0, this flag\'s 0.1) and '
+                  '--hidden_norm.  Only with --train_mode=pretrain.')
+    f.DEFINE_float('b200_gcl_lambda', 1.0, 'Weight of the distribution term of the generalized contrastive loss.')
+    f.DEFINE_float('b200_gcl_loss_scaling', 1.0, 'Scale of the generalized contrastive loss.')
 
 
 define_flags()

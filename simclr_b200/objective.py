@@ -145,6 +145,160 @@ def add_contrastive_loss(hidden, hidden_norm=True, temperature=1.0, strategy=Non
     return _NTXentFn.apply(hidden, hidden_norm, temperature, strategy)
 
 
+GCL_DISTS = ('logsumexp', 'normal', 'uniform')
+GCL_MAX_DIM = 256            # the tiled kernels keep a row of z in registers
+GCL_MAX_SORT_ROWS = 16384    # the sliced Wasserstein terms sort 2G keys per column in one CTA's shared memory
+
+
+def generalized_contrastive_dist():
+    """The `--b200_gcl_dist` of this run, or None when the pretraining objective is NT-Xent; raises ValueError
+    outside `--train_mode=pretrain`."""
+    from .flags_def import FLAGS
+    if FLAGS.b200_gcl_dist == 'none':
+        return None
+    if FLAGS.train_mode != 'pretrain':
+        raise ValueError('--b200_gcl_dist=%s needs --train_mode=pretrain (got %r): the generalized contrastive loss '
+                         'is a pretraining objective' % (FLAGS.b200_gcl_dist, FLAGS.train_mode))
+    return FLAGS.b200_gcl_dist
+
+
+def check_generalized_contrastive(dist, dim, global_rows):
+    """Raises ValueError for a configuration the kernels do not support: an unknown `dist`, D > 256, or, for the
+    sliced Wasserstein distributions, more than 16384 rows (2G) in the global batch."""
+    if dist not in GCL_DISTS:
+        raise ValueError('generalized contrastive loss: dist must be one of %s (got %r)' % (GCL_DISTS, dist))
+    if dim > GCL_MAX_DIM:
+        raise ValueError('generalized contrastive loss: the hidden dimension %d is above the supported %d'
+                         % (dim, GCL_MAX_DIM))
+    if dist != 'logsumexp' and global_rows > GCL_MAX_SORT_ROWS:
+        raise ValueError('generalized contrastive loss: dist=%r sorts %d rows (two views of the global batch) per '
+                         'column, above the supported %d' % (dist, global_rows, GCL_MAX_SORT_ROWS))
+
+
+def generalized_contrastive_forward(hidden, dist='normal', lambda_weight=1.0, temperature=1.0, hidden_norm=True,
+                                    loss_scaling=1.0, strategy=None, step=None, seed=0, draws=None):
+    """Forward of the generalized contrastive loss over the global batch; returns (loss, align, dist_loss, ctx).
+
+    hidden [2B, D] fp32, view-major.  `step` (an int, or a device int64 [1] that a captured graph reads on every
+    replay) and `seed` key the SWD draws: the prior [2G, D] and the orthogonal W [D, D], the same on every replica
+    for the same key.  `step=None` (one replica only) draws with a fresh key on every call, as the colab does; the
+    key's seed then comes from torch's default generator.  `draws=(W, prior)` replaces the draws (prior already
+    l2-normalised when hidden_norm); ctx.W and ctx.prior hold the draws of the call.  With more than one
+    replica the loss is this replica's L_r: the alignment over its rows, the logsumexp of its rows against all 2G
+    rows, or the SWD of all 2G rows (the same on every replica); the job's loss is the mean over replicas."""
+    e = get_engine()
+    assert hidden.dtype == torch.float32 and hidden.dim() == 2 and hidden.shape[0] % 2 == 0
+    hidden = hidden.contiguous()
+    rows, D = hidden.shape
+    B = rows // 2
+    R = strategy.num_replicas_in_sync if strategy is not None else 1
+    rid = strategy.replica_id if strategy is not None else 0
+    G = R * B
+    check_generalized_contrastive(dist, D, 2 * G)
+    st = stream_ptr()
+    z = e.empty((rows, D), torch.float32)
+    inv_norm = e.empty((rows,), torch.float32)
+    lib.ntxent_normalize(hidden, rows, D, int(bool(hidden_norm)), z, inv_norm, st)
+    z_all = strategy.all_gather(z, channel='z') if R > 1 else z            # [R][2][B][D]
+    ws_bytes = lib.gcl_workspace_bytes(B, R, D)
+    ws = e.empty((ws_bytes,), torch.uint8)
+    out = e.empty((3,), torch.float32)                                      # loss, align, dist
+    ctx = _Ctx()
+    ctx.dist, ctx.lse, ctx.perm, ctx.diff, ctx.W, ctx.prior, ctx.wnormal = dist, None, None, None, None, None, None
+    if dist == 'logsumexp':
+        ctx.lse = e.empty((rows,), torch.float32)
+        lib.gcl_lse_forward(z_all, B, R, D, rid, float(temperature), ctx.lse, out, ws, ws_bytes, st)
+    else:
+        if draws is None:
+            if step is None:
+                if R > 1:
+                    raise ValueError('generalized contrastive loss: with %d replicas the SWD draws must be the same on '
+                                     'every replica; pass the same step and seed on each' % R)
+                # a fresh key per call, reproducible through torch.manual_seed
+                seed, step = int(torch.randint(0, 2 ** 62, (1,)).item()), 0
+            if not torch.is_tensor(step):
+                step = torch.full((1,), int(step), dtype=torch.int64, device=e.device)
+            ctx.prior = e.empty((2 * G, D), torch.float32)
+            ctx.wnormal = e.empty((D, D), torch.float32)
+            ctx.W = e.empty((D, D), torch.float32)
+            lib.gcl_draw(int(seed), step, 2 * G, D, GCL_DISTS.index(dist) - 1, int(bool(hidden_norm)), ctx.prior,
+                         ctx.wnormal, st)
+            lib.gcl_orthogonal(ctx.wnormal, D, ctx.W, ws, ws_bytes, st)
+        else:
+            ctx.W, ctx.prior = (t.contiguous() for t in draws)
+            assert ctx.W.shape == (D, D) and ctx.prior.shape == (2 * G, D)
+        ctx.perm = e.empty((D, 2 * G), torch.int32)
+        ctx.diff = e.empty((D, 2 * G), torch.float32)
+        lib.gcl_swd_forward(z_all, ctx.prior, ctx.W, B, R, D, out, ctx.perm, ctx.diff, ws, ws_bytes, st)
+    ctx.dz_align = e.empty((rows, D), torch.float32)
+    lib.gcl_align(z, B, D, float(lambda_weight), float(loss_scaling), out, ctx.dz_align, st)
+    ctx.z, ctx.z_all, ctx.inv_norm, ctx.ws, ctx.ws_bytes = z, z_all, inv_norm, ws, ws_bytes
+    ctx.B, ctx.R, ctx.D, ctx.rid = B, R, D, rid
+    ctx.hidden_norm, ctx.temperature, ctx.strategy = bool(hidden_norm), float(temperature), strategy
+    ctx.lambda_weight, ctx.loss_scaling = float(lambda_weight), float(loss_scaling)
+    return out[0], out[1], out[2], ctx
+
+
+def generalized_contrastive_backward(ctx, grad_scale):
+    """d(job loss)/d(hidden) for this replica's rows.  grad_scale = d(job loss)/d(L_r), the same on every replica
+    (the step uses 1/R: loss / num_replicas, then the gradient sum).  The logsumexp key-side terms come from the
+    all-gathered lse; the SWD is the same on every replica, so each takes R times its weight for its own rows."""
+    e = get_engine()
+    st = stream_ptr()
+    B, R, D = ctx.B, ctx.R, ctx.D
+    w = float(grad_scale) * ctx.loss_scaling
+    dz_lse = dz_swd = None
+    if ctx.dist == 'logsumexp':
+        lse_all = ctx.strategy.all_gather(ctx.lse, channel='lse') if R > 1 else ctx.lse      # [R][2][B]
+        dz_lse = e.empty((2 * B, D), torch.float32)
+        lib.gcl_lse_backward(ctx.z_all, lse_all, B, R, D, ctx.rid, ctx.temperature, dz_lse, ctx.ws, ctx.ws_bytes, st)
+    else:
+        dz_swd = e.empty((2 * B, D), torch.float32)
+        lib.gcl_swd_backward(ctx.perm, ctx.diff, ctx.W, B, R, D, ctx.rid, dz_swd, ctx.ws, ctx.ws_bytes, st)
+    dhidden = e.empty((2 * B, D), torch.float32)
+    lib.gcl_normalize_backward(ctx.z, ctx.inv_norm, int(ctx.hidden_norm), 2 * B, D, ctx.dz_align, w,
+                               dz_lse, w * ctx.lambda_weight / (2 * B), dz_swd, w * ctx.lambda_weight * R, dhidden, st)
+    return dhidden
+
+
+class _GCLFn(torch.autograd.Function):
+    @staticmethod
+    def forward(fctx, hidden, lambda_weight, temperature, dist, hidden_norm, loss_scaling, strategy, step, seed):
+        loss, _, _, ctx = generalized_contrastive_forward(hidden, dist, lambda_weight, temperature, hidden_norm,
+                                                          loss_scaling, strategy, step, seed)
+        fctx.ctx = ctx
+        return loss
+
+    @staticmethod
+    def backward(fctx, g_loss):
+        # g_loss is this replica's weight; the job's gradient is the sum over replicas of equal weights
+        d = generalized_contrastive_backward(fctx.ctx, 1.0)
+        return (d * g_loss,) + (None,) * 8
+
+
+def generalized_contrastive_loss(hidden1, hidden2, lambda_weight=1.0, temperature=1.0, dist='normal',
+                                 hidden_norm=True, loss_scaling=1.0, strategy=None, step=None, seed=0):
+    """The intriguing-properties colab's `generalized_contrastive_loss` (Chen, Luo, Li 2021) on the H100 kernels.
+    Like the colab, every call draws a fresh W and prior unless `step` is given.
+
+    Args:
+      hidden1, hidden2: [B, D] fp32 hidden vectors of the two views.
+      lambda_weight: weight of the distribution-matching term.
+      temperature: temperature of the 'logsumexp' term.
+      dist: 'logsumexp' (decoupled NT-Xent), 'normal' or 'uniform' (sliced Wasserstein distance to that prior).
+      hidden_norm: whether to l2-normalise the hidden vectors (and the prior rows).
+      loss_scaling: scale of the whole loss.
+      strategy: replica context (`engine.ReplicaContext`) or None for one replica.
+      step, seed: key of the SWD draws (W and the prior): the same key gives the same draws on every replica.
+        None (one replica only): a fresh key on every call, its seed taken from torch's default generator.
+
+    Returns:
+      The loss scalar (this replica's L_r), differentiable with respect to hidden1 and hidden2.
+    """
+    return _GCLFn.apply(torch.cat([hidden1, hidden2], 0), lambda_weight, temperature, dist, hidden_norm,
+                        loss_scaling, strategy, step, seed)
+
+
 def tpu_cross_replica_concat(tensor, strategy=None):
     """tf2/objective.py:92-127: concatenation of `tensor` across replicas."""
     if strategy is None or strategy.num_replicas_in_sync <= 1:

@@ -41,9 +41,17 @@ class Trainer:
                 raise ValueError('the student has %d classes but the teacher %d: distilling across label spaces is '
                                  'not supported' % (num_classes, teacher.num_classes))
             num_classes = teacher.num_classes
+        # --b200_gcl_dist: the generalized contrastive loss replaces NT-Xent; its SWD draws are keyed by
+        # (seed, optimizer.iterations), staged in a device scalar so that graph replays draw anew
+        self.gcl = obj_lib.generalized_contrastive_dist()
+        self.seed = seed
         self.num_classes = num_classes or FLAGS.b200_num_classes
         self.num_examples = num_examples or FLAGS.b200_num_examples
         self.model = model_lib.Model(self.num_classes, seed=seed)
+        self._gcl_step = None
+        if self.gcl is not None:
+            obj_lib.check_generalized_contrastive(self.gcl, self._proj_dim(), 2 * FLAGS.train_batch_size)
+            self._gcl_step = torch.zeros(1, dtype=torch.int64, device=self.engine.device)
         self.learning_rate = model_lib.WarmUpAndCosineDecay(FLAGS.learning_rate, self.num_examples)
         self.optimizer = model_lib.build_optimizer(self.learning_rate)
         self.metrics = {}
@@ -132,7 +140,20 @@ class Trainer:
         B = features.shape[0]
         loss = None
         d_proj = d_sup = None
-        if projection_head_outputs is not None:
+        if projection_head_outputs is not None and self.gcl is not None:
+            if not torch.cuda.is_current_stream_capturing():
+                self.stage_gcl_step()
+            gcl_loss, align, dist_loss, ctx = obj_lib.generalized_contrastive_forward(
+                projection_head_outputs, self.gcl, FLAGS.b200_gcl_lambda, FLAGS.temperature, FLAGS.hidden_norm,
+                FLAGS.b200_gcl_loss_scaling, strategy=self.strategy if R > 1 else None, step=self._gcl_step,
+                seed=self.seed)
+            loss = gcl_loss
+            d_proj = obj_lib.generalized_contrastive_backward(ctx, 1.0 / R)
+            self.metrics['contrast_loss'] = gcl_loss
+            self.metrics['gcl_align_loss'] = align
+            self.metrics['gcl_dist_loss'] = dist_loss
+            self.metrics['gcl_draws'] = (ctx.W, ctx.prior)      # this step's SWD draws (None, None for logsumexp)
+        elif projection_head_outputs is not None:
             con_loss, logits_con, labels_con, ctx = obj_lib.contrastive_forward(
                 projection_head_outputs, hidden_norm=FLAGS.hidden_norm, temperature=FLAGS.temperature,
                 strategy=self.strategy if R > 1 else None, want_labels=False)
@@ -225,6 +246,7 @@ class Trainer:
         torch.cuda.current_stream().wait_stream(s)
         torch.cuda.synchronize()
         self.optimizer.stage_learning_rate()
+        self.stage_gcl_step()
         if R == 1:
             self._graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(self._graph):
@@ -262,12 +284,22 @@ class Trainer:
             return False
         if FLAGS.train_mode != 'pretrain':
             return True
-        head = self.model._projection_head.linear_layers
-        D = head[-1].num_classes if head else self.model.resnet_model.cout
         rows = features.shape[0] * (features.shape[3] // 3)
-        return gather_fits('z', rows * D * 4) and gather_fits('lse', rows * 4)
+        return gather_fits('z', rows * self._proj_dim() * 4) and gather_fits('lse', rows * 4)
+
+    def _proj_dim(self):
+        """Width of the projection head's output: the D of the contrastive objective."""
+        head = self.model._projection_head.linear_layers
+        return head[-1].num_classes if head else self.model.resnet_model.cout
+
+    def stage_gcl_step(self):
+        """Writes the step the next forward draws for (`optimizer.iterations`) into the device scalar the
+        generalized contrastive loss reads (stream-ordered fill; a no-op for NT-Xent)."""
+        if self._gcl_step is not None:
+            self._gcl_step.fill_(self.optimizer.iterations)
 
     def replay(self):
+        self.stage_gcl_step()
         self.optimizer.prepare_replay()
         self._graph.replay()
         if self._graph_apply is not None:
@@ -421,7 +453,14 @@ def main(argv):
     weight_decay_metric = metrics_lib.Mean('train/weight_decay')
     total_loss_metric = metrics_lib.Mean('train/total_loss')
     all_metrics = [weight_decay_metric, total_loss_metric]
-    if pretrain:
+    gcl = pretrain and trainer.gcl is not None
+    if gcl:
+        # the generalized contrastive loss has no NT-Xent logits: no contrast_acc / contrast_entropy
+        contrast_loss_metric = metrics_lib.Mean('train/contrast_loss')
+        gcl_align_metric = metrics_lib.Mean('train/gcl_align_loss')
+        gcl_dist_metric = metrics_lib.Mean('train/gcl_dist_loss')
+        all_metrics.extend([contrast_loss_metric, gcl_align_metric, gcl_dist_metric])
+    elif pretrain:
         contrast_loss_metric = metrics_lib.Mean('train/contrast_loss')
         contrast_acc_metric = metrics_lib.Mean('train/contrast_acc')
         contrast_entropy_metric = metrics_lib.Mean('train/contrast_entropy')
@@ -453,7 +492,11 @@ def main(argv):
             m = trainer.metrics
             weight_decay_metric.update_state(m['weight_decay'])
             total_loss_metric.update_state(m['total_loss'])
-            if pretrain:
+            if gcl:
+                contrast_loss_metric.update_state(m['contrast_loss'])
+                gcl_align_metric.update_state(m['gcl_align_loss'])
+                gcl_dist_metric.update_state(m['gcl_dist_loss'])
+            elif pretrain:
                 metrics_lib.update_pretrain_metrics_train(contrast_loss_metric, contrast_acc_metric, contrast_entropy_metric,
                                                           m['contrast_loss'], m['logits_con'], None,
                                                           trainer.strategy.replica_id)
