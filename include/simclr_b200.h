@@ -334,6 +334,13 @@ SIMCLR_API int simclr_pack_conv_weights_multi(const void* table_dev, int64_t n_l
  * memsets off with on = 1; returns the previous setting.  Process-wide, not thread-safe. */
 SIMCLR_API int simclr_set_accumulate_prezeroed(int on);
 SIMCLR_API int simclr_memset_zero(void* p, int64_t bytes, void* stream);
+/* 2-CTA TMA multicast in the implicit-GEMM and weight-gradient kernels of simclr_conv2d_*_tc: the two CTAs of a
+ * cluster read the operand tile they share from L2 once.  Outputs and fused sums are the same bits either way.
+ * Off by default (measured slower on ResNet-50, DESIGN.md 4.1); the environment variable SIMCLR_TC_MULTICAST=1
+ * sets the default to on.  Returns the previous setting.  Process-wide, not thread-safe. */
+SIMCLR_API int simclr_set_tc_multicast(int on);
+/* Clusters of `size` CTAs of the multicast conv kernels that the device holds at once (0 if it cannot). */
+SIMCLR_API int simclr_tc_max_active_clusters(int size);
 /* bn_sums (nullable): [2][Cout] doubles receiving sum y / sum y^2 of the stored outputs -- the
  * BatchNorm statistics of tf2/resnet.py:50-72 fused into the conv epilogue (zeroed by the call). */
 SIMCLR_API int simclr_conv2d_fprop_tc(const void* x, const void* wf, void* y, int dtype, int y_dtype,

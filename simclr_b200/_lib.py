@@ -70,7 +70,7 @@ def _conv(v, ct):
 # kernels launched per C-ABI call (for the `gpu_launches` claim of bench.py)
 _LAUNCHES = {'ntxent_forward': 3, 'ntxent_backward': 2, 'contrast_metrics': 3, 'softmax_xent': 2, 'l2_loss': 2,
              'lars_apply': 2, 'bn_bwd_apply': 2, 'version': 0, 'last_error': 0, 'ntxent_workspace_bytes': 0,
-             'set_accumulate_prezeroed': 0, 'memset_zero': 0, 'conv2d_fprop_tc3': 6, 'conv2d_dgrad_tc3': 6, 'conv2d_wgrad_tc3': 6,
+             'set_accumulate_prezeroed': 0, 'set_tc_multicast': 0, 'tc_max_active_clusters': 0, 'memset_zero': 0, 'conv2d_fprop_tc3': 6, 'conv2d_dgrad_tc3': 6, 'conv2d_wgrad_tc3': 6,
              'jpeg_decode': 3, 'distill_xent': 3, 'gcl_workspace_bytes': 0, 'gcl_lse_forward': 3,
              'gcl_lse_backward': 2, 'gcl_swd_forward': 5, 'gcl_swd_backward': 2}
 
@@ -120,7 +120,8 @@ class _Lib:
                 raise TypeError('%s expects %d arguments, got %d' % (full, len(cts), len(args)))
             r = fn(*[_conv(a, ct) for a, ct in zip(args, cts)])
             self.launch_count += nlaunch
-            if restype is ctypes.c_int and name not in ('version', 'set_accumulate_prezeroed'):
+            if restype is ctypes.c_int and name not in ('version', 'set_accumulate_prezeroed', 'set_tc_multicast',
+                                                        'tc_max_active_clusters'):
                 if r != 0:
                     raise SimclrError('%s failed with status %d: %s' % (full, r, self._dll.simclr_last_error().decode()))
                 return None

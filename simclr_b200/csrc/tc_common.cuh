@@ -61,6 +61,31 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------
+// Thread-block clusters
+// ---------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// Arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster.  CTA-scope release (the
+// default): the arrival only orders this CTA's completed reads of a stage before the peer's next TMA write into it.
+// A .release.cluster arrive compiles to MEMBAR.ALL.GPU, which would stall the consumer on every stage.
+__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n"
+      ".reg .b32 ra;\n"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n"
+      "}\n" ::"r"(smem_u32(bar)), "r"(cta)
+      : "memory");
+}
+// every thread of every CTA of the cluster: writes before the arrive are visible after the wait
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_sync() { cluster_arrive(); cluster_wait(); }
+
+// ---------------------------------------------------------------------------
 // TMA
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -70,6 +95,15 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"((uint64_t)tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+      : "memory");
+}
+// The same box written to the same shared-memory offset of every CTA in `cta_mask`; each destination's mbarrier
+// at `bar`'s offset receives the complete_tx of its copy.
+__device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, int c0, int c1,
+                                               uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_u32(smem_dst)), "l"((uint64_t)tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
 // fp32 pairs kept in one 64-bit register (the statistics loops' running sums)
@@ -96,6 +130,16 @@ __device__ __forceinline__ void tma_load_im2col(void* smem_dst, const CUtensorMa
   asm volatile(
       "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8};"
       ::"r"(smem_u32(smem_dst)), "l"((uint64_t)tmap), "r"(smem_u32(bar)), "r"(c), "r"(w), "r"(h), "r"(n), "h"(ow), "h"(oh)
+      : "memory");
+}
+// multicast form of tma_load_im2col (see tma_load_2d_mc)
+__device__ __forceinline__ void tma_load_im2col_mc(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, int c, int w,
+                                                   int h, int n, int off_w, int off_h, uint16_t cta_mask) {
+  const uint16_t ow = (uint16_t)off_w, oh = (uint16_t)off_h;
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5, %6}], [%2], {%7, %8}, %9;"
+      ::"r"(smem_u32(smem_dst)), "l"((uint64_t)tmap), "r"(smem_u32(bar)), "r"(c), "r"(w), "r"(h), "r"(n), "h"(ow), "h"(oh),
+        "h"(cta_mask)
       : "memory");
 }
 

@@ -9,6 +9,16 @@
 // Pipeline: smem full/empty mbarriers (producers <-> consumer); the producers run ahead into
 // the next tile while the consumer drains the accumulators.  Tiles: 128 x BN x 128 bytes of K
 // per stage, BN <= 128 (a 128 x 128 fp32 accumulator is 128 registers per consumer thread).
+//
+// Multicast (MC): CTAs 2c and 2c+1 form a cluster and, on every iteration of the persistent loop, hold work items
+// that share one operand tile (A: same rows, adjacent column blocks; B: adjacent row blocks, one column block).
+// Each loads half of the shared tile and multicasts it to both, so the pair reads it from L2 once.  A CTA's full[s]
+// expects the same bytes as without multicast; its empty[s] counts the consumer warps of both CTAs, because the
+// peer's producer writes into stage s.  An iteration is paired only when both CTAs have an item; the unpaired tail
+// loads privately and its stages are released twice locally.  Cluster barriers after the mbarrier init and before
+// exit keep a CTA from writing into a peer that has not started or has already left.
+#include <utility>
+
 #include "tc_common.cuh"
 
 namespace simclr {
@@ -74,6 +84,7 @@ struct Geom {
   // (q*stride + im_base, p*stride + im_base); the tap goes into the instruction's filter offsets
   int im2col, im_base, im_nimg;
   int accum;           // fp32 outputs only: add into `out` (TMA reduce-add / atomics) instead of storing (tc3 passes)
+  int mc;              // 2-CTA multicast: 0 off, 1 the pair shares the A (X) tile, 2 the B (dY) tile
 };
 
 template <typename T> struct Elt;
@@ -139,6 +150,19 @@ __device__ __forceinline__ void warp_arrive(uint64_t* bar) {
   __syncwarp();
   if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
 }
+// A consumer warp hands stage `bar` back.  With multicast empty[s] counts both CTAs' warps: a paired stage is
+// released on this CTA and on the peer, whose producer wrote half of it; an unpaired one counts twice here.
+template <bool MC>
+__device__ __forceinline__ void release_stage(uint64_t* bar, bool paired, uint32_t peer) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) {
+    mbar_arrive(bar);
+    if (MC) {
+      if (paired) mbar_arrive_remote(bar, peer);
+      else mbar_arrive(bar);
+    }
+  }
+}
 
 struct SmemCtl {
   uint64_t* full; uint64_t* empty;
@@ -158,7 +182,7 @@ __device__ __forceinline__ SmemCtl carve(uint8_t* base, int stage_bytes) {
 // ===========================================================================
 // fprop / dgrad / dense:  out[M][n_out] = gather(src)[M][K] * Wk[n_out][K]^T
 // ===========================================================================
-template <typename T, typename To, int BN, bool A_TMA, bool SMALLC, bool TMA_EPI, bool STATS>
+template <typename T, typename To, int BN, bool A_TMA, bool SMALLC, bool TMA_EPI, bool STATS, bool MC>
 __global__ void __launch_bounds__(igemm_threads(A_TMA, STATS), 1)
 igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
              const __grid_constant__ CUtensorMap tmap_out, const Geom g, double* __restrict__ bn_sums) {
@@ -168,16 +192,18 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
   constexpr int KBE = Elt<T>::KBE;
   constexpr int CH = Elt<T>::CH;
   constexpr int NF = BN / 2;                          // accumulator registers per thread and m64 half
+  static_assert(!MC || A_TMA, "multicast needs both operands fed by TMA");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const SmemCtl ctl = carve<STAGES>(smem, TL::STAGE_BYTES);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t rank = MC ? cluster_ctarank() : 0;   // clusters of 2 along x: rank == blockIdx.x & 1
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&ctl.full[s], A_TMA ? 1 : 1 + GATHER_THREADS / 32);
-      mbar_init(&ctl.empty[s], EPI_THREADS / 32);
+      mbar_init(&ctl.empty[s], (MC ? 2 : 1) * EPI_THREADS / 32);
     }
     for (int a = 0; a < 2; ++a) { mbar_init(&ctl.sfull[a], 1); mbar_init(&ctl.sfree[a], STATS_THREADS / 32); }
     fence_barrier_init();
@@ -193,7 +219,8 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
   constexpr int BOX_COLS = 128 / (int)sizeof(To);     // 64 (bf16) / 32 (fp32) output columns per staged tile
   constexpr int BOXES = BN / BOX_COLS;
   constexpr int CPC = 16 / (int)sizeof(To);           // columns per 16-byte chunk: 8 (bf16) / 4 (fp32)
-  __syncthreads();
+  if (MC) cluster_sync();                             // the peer's barriers exist before anything lands on them
+  else __syncthreads();
   const int num_tiles = g.tiles_m * g.tiles_n;
 
   if (warp < 4) {
@@ -221,6 +248,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
     const bool vec_ok = ((reinterpret_cast<uintptr_t>(out) & 15) == 0) && ((g.ldc * (int)sizeof(To)) % 16 == 0);
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int tm = tile / g.tiles_n, tn = tile - tm * g.tiles_n;
+      const bool paired = MC && tile - (int)rank + 1 < num_tiles;   // the same value on both CTAs of the pair
       int prev = 0;
       for (int kb = 0; kb < g.num_kb; ++kb) {
         mbar_wait(&ctl.full[pp.stage], pp.phase);
@@ -234,12 +262,12 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
             wgmma<BN, TF32, false, false>(acc[h], desc_pack(a_lo + h * (64 * 128 >> 4) + 2 * k, HI), desc_pack(b_lo + 2 * k, HI),
                                           (kb | k) != 0 ? 1u : 0u);
         wgmma_commit();
-        if (kb > 0) { wgmma_wait<1>(); warp_arrive(&ctl.empty[prev]); }
+        if (kb > 0) { wgmma_wait<1>(); release_stage<MC>(&ctl.empty[prev], paired, rank ^ 1); }
         prev = pp.stage;
         advance<STAGES>(pp);
       }
       wgmma_wait<0>(acc);
-      warp_arrive(&ctl.empty[prev]);
+      release_stage<MC>(&ctl.empty[prev], paired, rank ^ 1);
 
       if (TMA_EPI) {
         // registers -> 128B-swizzled smem tile [128 rows][128 B] -> TMA store (coalesced, rows >= M and
@@ -342,35 +370,56 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
     // ------------------------------ TMA producer --------------------------
     if (lane == 0) {
       Pipe pp{0, 0};
+      // With a shared tile the tensor map's box is half of it (64 A rows or BN/2 B rows): a paired CTA loads its
+      // half for both CTAs, an unpaired one both halves for itself.
+      const bool share_a = MC && g.mc == 1, share_b = MC && g.mc == 2;
+      const int a_parts = share_a ? 2 : 1, b_parts = share_b ? 2 : 1;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const int tm = tile / g.tiles_n, tn = tile - tm * g.tiles_n;
-        // im2col feed: base pixel of the tile's first row; taps advance in K order, cblocks channel blocks each
-        int im_n = 0, im_w = 0, im_h = 0, tap = 0, cb = 0, tr = 0, ts = 0;
+        const bool paired = MC && tile - (int)rank + 1 < num_tiles;
+        // im2col feed: base pixel of the first row of each A box; taps advance in K order, cblocks channel blocks each
+        int im_n[2] = {0, 0}, im_w[2] = {0, 0}, im_h[2] = {0, 0}, tap = 0, cb = 0, tr = 0, ts = 0;
         if (A_TMA && g.im2col) {
-          uint32_t n, rem, p, q;
-          g.dPQ.divmod((uint32_t)(tm * 128), n, rem);
-          g.dQ.divmod(rem, p, q);
-          im_n = (int)n; im_w = (int)q * g.stride + g.im_base; im_h = (int)p * g.stride + g.im_base;
+          for (int h = 0; h < a_parts; ++h) {
+            uint32_t n, rem, p, q;
+            g.dPQ.divmod((uint32_t)(tm * 128 + h * 64), n, rem);
+            g.dQ.divmod(rem, p, q);
+            im_n[h] = (int)n; im_w[h] = (int)q * g.stride + g.im_base; im_h[h] = (int)p * g.stride + g.im_base;
+          }
         }
         for (int kb = 0; kb < g.num_kb; ++kb) {
           mbar_wait(&ctl.empty[pp.stage], pp.phase ^ 1);
           uint8_t* a_dst = smem + (size_t)pp.stage * TL::STAGE_BYTES;
-          mbar_arrive_expect_tx(&ctl.full[pp.stage], TL::B_STAGE_BYTES + (A_TMA ? A_STAGE_BYTES : 0));
+          uint64_t* full = &ctl.full[pp.stage];
+          mbar_arrive_expect_tx(full, TL::B_STAGE_BYTES + (A_TMA ? A_STAGE_BYTES : 0));
           if (A_TMA) {
+            int ow = 0, oh = 0;
             if (g.im2col) {
-              int ow, oh;
               if (g.use_tab) { ow = g.tab_s[tap] - g.im_base; oh = g.tab_r[tap] - g.im_base; }
               else if (g.tap_sign > 0) { ow = ts; oh = tr; }
               else { ow = g.S - 1 - ts; oh = g.R - 1 - tr; }
-              tma_load_im2col(a_dst, &tmap_a, &ctl.full[pp.stage], cb * KBE, im_w, im_h, im_n, ow, oh);
-              if (++cb == g.cblocks) { cb = 0; ++tap; if (++ts == g.S) { ts = 0; ++tr; } }
-            } else {
-              tma_load_2d(a_dst, &tmap_a, &ctl.full[pp.stage], kb * KBE, tm * 128);
             }
+            for (int h = 0; h < a_parts; ++h) {
+              if (share_a && paired && h != (int)rank) continue;
+              uint8_t* dst = a_dst + h * (A_STAGE_BYTES / 2);
+              if (g.im2col) {
+                if (share_a && paired) tma_load_im2col_mc(dst, &tmap_a, full, cb * KBE, im_w[h], im_h[h], im_n[h], ow, oh, 0x3);
+                else tma_load_im2col(dst, &tmap_a, full, cb * KBE, im_w[h], im_h[h], im_n[h], ow, oh);
+              } else {
+                if (share_a && paired) tma_load_2d_mc(dst, &tmap_a, full, kb * KBE, tm * 128 + h * 64, 0x3);
+                else tma_load_2d(dst, &tmap_a, full, kb * KBE, tm * 128 + h * 64);
+              }
+            }
+            if (g.im2col && ++cb == g.cblocks) { cb = 0; ++tap; if (++ts == g.S) { ts = 0; ++tr; } }
           }
           int kcol = kb * KBE;
           if (g.use_tab) { const int t = kb / g.cblocks; kcol = g.tab_kcol[t] + (kb - t * g.cblocks) * KBE; }
-          tma_load_2d(a_dst + A_STAGE_BYTES, &tmap_b, &ctl.full[pp.stage], kcol, tn * BN);
+          for (int h = 0; h < b_parts; ++h) {
+            if (share_b && paired && h != (int)rank) continue;
+            uint8_t* dst = a_dst + A_STAGE_BYTES + h * (TL::B_STAGE_BYTES / 2);
+            if (share_b && paired) tma_load_2d_mc(dst, &tmap_b, full, kcol, tn * BN + h * (BN / 2), 0x3);
+            else tma_load_2d(dst, &tmap_b, full, kcol, tn * BN + h * (BN / 2));
+          }
           advance<STAGES>(pp);
         }
       }
@@ -522,7 +571,8 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
     }
   }
 
-  __syncthreads();
+  if (MC) cluster_sync();       // the peer may still arrive on this CTA's barriers until it gets here
+  else __syncthreads();
 }
 
 // ===========================================================================
@@ -531,7 +581,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
 // Work item = (128 k-rows) x (BN couts) x (pixel split).  With one split every dW element is written once; with
 // several, each split writes its partial to scratch and run_sum_partials adds them in split order (deterministic).
 // ===========================================================================
-template <typename T, int BN, bool SMALLC, bool A_TMA, bool TMA_RED>
+template <typename T, int BN, bool SMALLC, bool A_TMA, bool TMA_RED, bool MC>
 __global__ void __launch_bounds__(wgrad_threads(A_TMA), 1)
 wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_dy,
              const __grid_constant__ CUtensorMap tmap_dw, const Geom g, float* __restrict__ dw) {
@@ -548,14 +598,19 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
   constexpr int NF = BN / 2;
   static_assert(PXS / MMA_K == 4, "4 MMAs per stage");
   static_assert(A_ATOMS == 2, "one 64-row atom per m64 half");
+  static_assert(!MC || A_TMA, "multicast needs both operands fed by TMA");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const SmemCtl ctl = carve<STAGES>(smem, TL::STAGE_BYTES);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t rank = MC ? cluster_ctarank() : 0;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&ctl.full[s], A_TMA ? 1 : 1 + GATHER_THREADS / 32); mbar_init(&ctl.empty[s], EPI_THREADS / 32); }
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&ctl.full[s], A_TMA ? 1 : 1 + GATHER_THREADS / 32);
+      mbar_init(&ctl.empty[s], (MC ? 2 : 1) * EPI_THREADS / 32);
+    }
     fence_barrier_init();
   }
   if (warp == 4 && lane == 0) {
@@ -563,13 +618,21 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
     if (A_TMA) tma_prefetch_desc(&tmap_x);
     if (TMA_RED) tma_prefetch_desc(&tmap_dw);
   }
-  __syncthreads();
+  if (MC) cluster_sync();
+  else __syncthreads();
   const int num_items = g.tiles_m * g.tiles_n * g.splits;   // tiles_m = k-row tiles
 
-  // item -> (tk, tn, split); splits of one tile are adjacent so their dY reads share L2
-  auto decode = [&](int item, int& tk, int& tn, int& kb0, int& kb1) {
-    const int split = item % g.splits;
-    const int t = item / g.splits;
+  // item -> (tk, tn, split), the split outermost: the CTAs that run at the same time take every tile of one pixel
+  // range, so the X and dY pixel blocks those tiles share are re-read while they are still in L2.  With the splits
+  // of one tile side by side they were read waves apart, and the ResNet-50 wgrad launches took 25 % longer (H100
+  // SXM, DESIGN.md 4.1).  With multicast, items 2i and 2i + 1 are then (tk, tn), (tk, tn + 1) of one split
+  // (tiles_n even: they share X) or, with one column block, (tk, tn), (tk + 1, tn) (tiles_m even: they share dY).
+  // The item -> CTA map changes no bit: split partials are summed in split order, and a single-split tile gets
+  // one reduce-add.
+  auto decode = [&](int item, int& tk, int& tn, int& split, int& kb0, int& kb1) {
+    const int tiles = g.tiles_m * g.tiles_n;
+    split = item / tiles;
+    const int t = item - split * tiles;
     tk = t / g.tiles_n; tn = t - tk * g.tiles_n;
     kb0 = split * g.kb_per_split;
     kb1 = min(g.num_kb, kb0 + g.kb_per_split);
@@ -586,9 +649,9 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
     Pipe pp{0, 0};
     uint32_t box_ctr = 0;
     for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-      int tk, tn, kb0, kb1; decode(item, tk, tn, kb0, kb1);
+      int tk, tn, split, kb0, kb1; decode(item, tk, tn, split, kb0, kb1);
       if (kb0 >= kb1) continue;
-      const int split = item % g.splits;
+      const bool paired = MC && item - (int)rank + 1 < num_items;   // the same value on both CTAs of the pair
       int prev = 0;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&ctl.full[pp.stage], pp.phase);
@@ -602,12 +665,12 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
             wgmma<BN, false, true, true>(acc[h], desc_pack(a_lo + h * (ATOM_BYTES >> 4) + k * (MMA_K * 128 >> 4), HI),
                                          desc_pack(b_lo + k * (MMA_K * 128 >> 4), HI), (kb > kb0 || k > 0) ? 1u : 0u);
         wgmma_commit();
-        if (kb > kb0) { wgmma_wait<1>(); warp_arrive(&ctl.empty[prev]); }
+        if (kb > kb0) { wgmma_wait<1>(); release_stage<MC>(&ctl.empty[prev], paired, rank ^ 1); }
         prev = pp.stage;
         advance<STAGES>(pp);
       }
       wgmma_wait<0>(acc);
-      warp_arrive(&ctl.empty[prev]);
+      release_stage<MC>(&ctl.empty[prev], paired, rank ^ 1);
       if (TMA_RED) {
         // partial tile -> swizzled smem [128 k-rows][32 fp32] -> TMA reduce-add into dW, or TMA store into this
         // split's rows of the scratch partials
@@ -666,12 +729,16 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
     if (lane == 0) {
       Pipe pp{0, 0};
       for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-        int tk, tn, kb0, kb1; decode(item, tk, tn, kb0, kb1);
+        int tk, tn, split, kb0, kb1; decode(item, tk, tn, split, kb0, kb1);
+        // a paired CTA loads atom `rank` of the shared tile (X, or dY with g.mc == 2) for both CTAs
+        const bool paired = MC && item - (int)rank + 1 < num_items;
+        const bool mc_x = paired && g.mc == 1, mc_dy = paired && g.mc == 2;
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&ctl.empty[pp.stage], pp.phase ^ 1);
           uint8_t* a_dst = smem + (size_t)pp.stage * TL::STAGE_BYTES;
           uint8_t* b_dst = a_dst + TL::A_BYTES;
-          mbar_arrive_expect_tx(&ctl.full[pp.stage], TL::B_STAGE_BYTES + (A_TMA ? TL::A_BYTES : 0));
+          uint64_t* full = &ctl.full[pp.stage];
+          mbar_arrive_expect_tx(full, TL::B_STAGE_BYTES + (A_TMA ? TL::A_BYTES : 0));
           if (A_TMA) {
             if (g.im2col) {  // one im2col column of PXS pixels per atom: the atom's tap is the filter offset
               uint32_t n, rem, p, q;
@@ -679,23 +746,31 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
               g.dQ.divmod(rem, p, q);
 #pragma unroll
               for (int a = 0; a < A_ATOMS; ++a) {
+                if (mc_x && a != (int)rank) continue;
                 uint32_t tap, c, r, s2;
                 g.dC.divmod((uint32_t)(tk * 128 + a * ATOM_E), tap, c);
                 g.dS.divmod(tap, r, s2);
                 const bool live = (int)tap < g.RS;     // k-rows past R*S*C: read a non-existent image (zeros)
-                tma_load_im2col(a_dst + a * ATOM_BYTES, &tmap_x, &ctl.full[pp.stage], (int)c,
-                                (int)q * g.stride + g.im_base, (int)p * g.stride + g.im_base,
-                                live ? (int)n : g.im_nimg, live ? (int)s2 : 0, live ? (int)r : 0);
+                const int iw = (int)q * g.stride + g.im_base, ih = (int)p * g.stride + g.im_base;
+                const int in = live ? (int)n : g.im_nimg, ow = live ? (int)s2 : 0, oh = live ? (int)r : 0;
+                if (mc_x) tma_load_im2col_mc(a_dst + a * ATOM_BYTES, &tmap_x, full, (int)c, iw, ih, in, ow, oh, 0x3);
+                else tma_load_im2col(a_dst + a * ATOM_BYTES, &tmap_x, full, (int)c, iw, ih, in, ow, oh);
               }
             } else {         // 1x1 stride-1: the activation tile is a plain [pixels][channels] box
 #pragma unroll
-              for (int a = 0; a < A_ATOMS; ++a)
-                tma_load_2d(a_dst + a * ATOM_BYTES, &tmap_x, &ctl.full[pp.stage], tk * 128 + a * ATOM_E, kb * PXS);
+              for (int a = 0; a < A_ATOMS; ++a) {
+                if (mc_x && a != (int)rank) continue;
+                if (mc_x) tma_load_2d_mc(a_dst + a * ATOM_BYTES, &tmap_x, full, tk * 128 + a * ATOM_E, kb * PXS, 0x3);
+                else tma_load_2d(a_dst + a * ATOM_BYTES, &tmap_x, full, tk * 128 + a * ATOM_E, kb * PXS);
+              }
             }
           }
 #pragma unroll
-          for (int a = 0; a < B_ATOMS; ++a)
-            tma_load_2d(b_dst + a * ATOM_BYTES, &tmap_dy, &ctl.full[pp.stage], tn * BN + a * ATOM_E, kb * PXS);
+          for (int a = 0; a < B_ATOMS; ++a) {
+            if (mc_dy && a != (int)rank) continue;
+            if (mc_dy) tma_load_2d_mc(b_dst + a * ATOM_BYTES, &tmap_dy, full, tn * BN + a * ATOM_E, kb * PXS, 0x3);
+            else tma_load_2d(b_dst + a * ATOM_BYTES, &tmap_dy, full, tn * BN + a * ATOM_E, kb * PXS);
+          }
           advance<STAGES>(pp);
         }
       }
@@ -708,7 +783,7 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
     Pipe pi{0, 0}, pa{0, 0};
     int inflight = 0;
     for (int item = blockIdx.x; item < num_items; item += gridDim.x) {
-      int tk, tn, kb0, kb1; decode(item, tk, tn, kb0, kb1);
+      int tk, tn, split, kb0, kb1; decode(item, tk, tn, split, kb0, kb1);
       // piece i of this thread: q = gt/8 + GROWS*i -> atom q / PXS, pixel q % PXS; its (tap, c) is fixed per item
       int pdr[GPT], pds[GPT], pc[GPT]; bool pk[GPT];
       int pdr2[GPT], pds2[GPT]; bool pk2[GPT];
@@ -793,7 +868,8 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
     for (; inflight > 0; --inflight) { warp_arrive(&ctl.full[pa.stage]); advance<STAGES>(pa); }
   }
 
-  __syncthreads();
+  if (MC) cluster_sync();
+  else __syncthreads();
 }
 
 // ---------------------------------------------------------------------------
@@ -818,23 +894,67 @@ inline int igemm_grid(const Geom& g, bool stats) {
   return grid;
 }
 
-template <typename T, typename To, int BN, bool A_TMA, bool SMALLC, bool TMA_EPI, bool STATS>
-int launch_igemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout, const Geom& g, double* bn_sums,
-                 cudaStream_t st) {
-  auto kern = igemm_kernel<T, To, BN, A_TMA, SMALLC, TMA_EPI, STATS>;
-  { int rc = set_smem_attr(kern, Tile<BN>::SMEM_BYTES); if (rc) return rc; }   // a per-DEVICE attribute: set on every launch
-  const int grid = igemm_grid(g, STATS);
-  kern<<<grid, igemm_threads(A_TMA, STATS), Tile<BN>::SMEM_BYTES, st>>>(ta, tb, tout, g, bn_sums);
+// 2-CTA multicast of the shared operand tile: off unless SIMCLR_TC_MULTICAST=1 or simclr_set_tc_multicast(1).  It
+// gives the same bits and measured slower on ResNet-50 (DESIGN.md 4.1); it stays as the A/B arm of that measurement.
+static int g_multicast = -1;
+inline bool multicast_enabled() {
+  if (g_multicast < 0) { const char* e = getenv("SIMCLR_TC_MULTICAST"); g_multicast = (e && e[0] == '1') ? 1 : 0; }
+  return g_multicast == 1;
+}
+// Clusters of `size` CTAs of the multicast kernels that fit on the device at once (every operand-ring kernel takes
+// one SM's shared memory, so the figure holds for all of them); 0 if the query fails.
+int max_active_clusters(int size);
+// Pairs the persistent grid can hold at once, queried once per process.  A multicast launch needs its whole grid
+// co-resident: otherwise the last clusters would wait for a second wave and the launch would be slower.
+inline int cluster_pairs() {
+  static int n = -1;
+  if (n < 0) n = max_active_clusters(2);
+  return n;
+}
+// What the CTA pairs of a persistent launch share (Geom::mc): items 2i and 2i + 1 of the loop take adjacent column
+// blocks of the same rows when tiles_n is even (A), or adjacent row blocks when there is one column block (B).
+// `b_ok` is false where the B tile cannot be split into two halves.
+inline int plan_multicast(int grid, int tiles_m, int tiles_n, bool b_ok) {
+  if (!multicast_enabled() || grid % 2 != 0 || grid / 2 > cluster_pairs()) return 0;
+  if (tiles_n % 2 == 0) return 1;
+  if (tiles_n == 1 && tiles_m > 1 && b_ok) return 2;
+  return 0;
+}
+
+// Grid of `grid` CTAs; with `pairs` consecutive CTAs form clusters of 2 (multicast kernels).
+template <typename... P, typename... A>
+int launch_kernel(void (*kern)(P...), int grid, int threads, size_t smem, bool pairs, cudaStream_t st, A&&... args) {
+  if (!pairs) {
+    kern<<<grid, threads, smem, st>>>(std::forward<A>(args)...);
+  } else {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid); cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = 2; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr; cfg.numAttrs = 1;
+    cudaLaunchKernelEx(&cfg, kern, std::forward<A>(args)...);
+  }
   SIMCLR_CHECK_LAUNCH();
   return SIMCLR_OK;
+}
+
+template <typename T, typename To, int BN, bool A_TMA, bool SMALLC, bool TMA_EPI, bool STATS, bool MC>
+int launch_igemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout, const Geom& g, double* bn_sums,
+                 cudaStream_t st) {
+  auto kern = igemm_kernel<T, To, BN, A_TMA, SMALLC, TMA_EPI, STATS, MC>;
+  { int rc = set_smem_attr(kern, Tile<BN>::SMEM_BYTES); if (rc) return rc; }   // a per-DEVICE attribute: set on every launch
+  return launch_kernel(kern, igemm_grid(g, STATS), igemm_threads(A_TMA, STATS), Tile<BN>::SMEM_BYTES, MC, st, ta, tb, tout, g,
+                       bn_sums);
 }
 
 template <typename T, typename To, int BN, bool TMA_EPI, bool STATS>
 int dispatch_igemm3(bool a_tma, bool smallc, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout,
                     const Geom& g, double* bn_sums, cudaStream_t st) {
-  if (a_tma) return launch_igemm<T, To, BN, true, false, TMA_EPI, STATS>(ta, tb, tout, g, bn_sums, st);
-  if (smallc) return launch_igemm<T, To, BN, false, true, TMA_EPI, STATS>(ta, tb, tout, g, bn_sums, st);
-  return launch_igemm<T, To, BN, false, false, TMA_EPI, STATS>(ta, tb, tout, g, bn_sums, st);
+  if (a_tma && g.mc) return launch_igemm<T, To, BN, true, false, TMA_EPI, STATS, true>(ta, tb, tout, g, bn_sums, st);
+  if (a_tma) return launch_igemm<T, To, BN, true, false, TMA_EPI, STATS, false>(ta, tb, tout, g, bn_sums, st);
+  if (smallc) return launch_igemm<T, To, BN, false, true, TMA_EPI, STATS, false>(ta, tb, tout, g, bn_sums, st);
+  return launch_igemm<T, To, BN, false, false, TMA_EPI, STATS, false>(ta, tb, tout, g, bn_sums, st);
 }
 template <typename T, typename To, int BN>
 int dispatch_igemm2(bool a_tma, bool smallc, bool tma_epi, const CUtensorMap& ta, const CUtensorMap& tb,
@@ -941,22 +1061,24 @@ int run_igemm(int mode, const void* src, const void* wk, void* out, int dtype, i
   g.use_tab = 0; g.cblocks = 1; g.os = 0; g.oh0 = g.ow0 = 0; g.OH = g.OW = 0;
   g.tap_sign = mode == 0 ? 1 : -1;
   g.im2col = 0; g.im_base = 0; g.im_nimg = (int)N; g.accum = accum ? 1 : 0;
-  // plain GEMM (1x1, stride 1, no padding): activations go through TMA as well
-  bool a_tma = (R == 1 && S == 1 && stride == 1 && !smallc && (Cs * es) % 16 == 0);
+  // plain GEMM (1x1, stride 1, no padding): activations go through TMA as well; every other shape with whole
+  // 128-byte channel blocks through TMA im2col (square filter, symmetric padding)
+  const bool a_2d = (R == 1 && S == 1 && stride == 1 && !smallc && (Cs * es) % 16 == 0);
+  Im2colPlan pl;
+  const bool a_im2col = !a_2d && !smallc && plan_im2col(mode, Hs, Ws, Cs, P, Q, R, S, stride, KBE, &pl);
+  const bool a_tma = a_2d || a_im2col;
+  g.mc = a_tma ? plan_multicast(igemm_grid(g, bn_sums != nullptr), g.tiles_m, g.tiles_n, true) : 0;
+  const uint32_t a_box = g.mc == 1 ? 64 : 128, b_box = g.mc == 2 ? bn / 2 : bn;   // a shared tile is loaded in halves
   CUtensorMap ta, tb, tout;
-  int rc = make_tmap_2d(&tb, wk, es, (uint64_t)n_out, (uint64_t)Kp, (uint64_t)Kp * es, (uint32_t)bn, (uint32_t)KBE);
+  int rc = make_tmap_2d(&tb, wk, es, (uint64_t)n_out, (uint64_t)Kp, (uint64_t)Kp * es, b_box, (uint32_t)KBE);
   if (rc) return rc;
-  if (a_tma) { rc = make_tmap_2d(&ta, src, es, (uint64_t)M, (uint64_t)Cs, (uint64_t)Cs * es, 128, (uint32_t)KBE); if (rc) return rc; }
-  else {
+  if (a_2d) { rc = make_tmap_2d(&ta, src, es, (uint64_t)M, (uint64_t)Cs, (uint64_t)Cs * es, a_box, (uint32_t)KBE); if (rc) return rc; }
+  else if (a_im2col) {
+    rc = make_tmap_im2col(&ta, src, es, (uint64_t)N, (uint64_t)Hs, (uint64_t)Ws, (uint64_t)Cs, pl.lo, pl.up, (uint32_t)stride, a_box);
+    if (rc) return rc;
+    g.im2col = 1; g.im_base = pl.lo; g.cblocks = (int)(Cs / KBE);
+  } else {
     ta = tb;
-    // every other shape with whole 128-byte channel blocks: TMA im2col (square filter, symmetric padding)
-    Im2colPlan pl;
-    if (!smallc && plan_im2col(mode, Hs, Ws, Cs, P, Q, R, S, stride, KBE, &pl)) {
-      rc = make_tmap_im2col(&ta, src, es, (uint64_t)N, (uint64_t)Hs, (uint64_t)Ws, (uint64_t)Cs, pl.lo, pl.up, (uint32_t)stride, 128);
-      if (rc) return rc;
-      g.im2col = 1; g.im_base = pl.lo; g.cblocks = (int)(Cs / KBE);
-      a_tma = true;
-    }
   }
   // coalesced TMA-store epilogue whenever the output rows are 16-byte aligned
   const int eo = out_dtype == SIMCLR_BF16 ? 2 : 4;
@@ -1057,22 +1179,28 @@ int run_dgrad_strided(const void* dy, const void* wd, void* dx, int dtype, int o
       g.use_tab = 1; g.os = (int)stride; g.oh0 = ph; g.ow0 = pw; g.OH = (int)H; g.OW = (int)W;
       // the class is a stride-1 walk over the dY grid: TMA im2col when its pixel grid is the dY grid
       g.im2col = 0; g.im_base = 0; g.im_nimg = (int)N; g.accum = accum ? 1 : 0;
-      CUtensorMap ta = tb;
+      CUtensorMap ta = tb, tbc = tb;
       bool a_tma = false;
+      g.mc = 0;
       if (im2col_enabled() && get_encode_im2col() != nullptr && P2 == Ho && Q2 == Wo && Ho < 32768 && Wo < 32768) {
         int lo = g.tab_r[0];
         for (int t = 0; t < nt; ++t) { lo = g.tab_r[t] < lo ? g.tab_r[t] : lo; lo = g.tab_s[t] < lo ? g.tab_s[t] : lo; }
         int hi = lo;
         for (int t = 0; t < nt; ++t) { hi = g.tab_r[t] > hi ? g.tab_r[t] : hi; hi = g.tab_s[t] > hi ? g.tab_s[t] : hi; }
         if (lo >= -128 && hi - lo <= 255) {
-          rc = make_tmap_im2col(&ta, dy, es, (uint64_t)N, (uint64_t)Ho, (uint64_t)Wo, (uint64_t)Cout, lo, lo, 1, 128);
+          g.mc = plan_multicast(igemm_grid(g, false), g.tiles_m, g.tiles_n, true);
+          rc = make_tmap_im2col(&ta, dy, es, (uint64_t)N, (uint64_t)Ho, (uint64_t)Wo, (uint64_t)Cout, lo, lo, 1, g.mc == 1 ? 64 : 128);
           if (rc) return rc;
+          if (g.mc == 2) {      // the class's B tile is loaded in halves
+            rc = make_tmap_2d(&tbc, wd, es, (uint64_t)Cin, (uint64_t)Kdp, (uint64_t)Kdp * es, (uint32_t)bn / 2, (uint32_t)KBE);
+            if (rc) return rc;
+          }
           g.im2col = 1; g.im_base = lo; a_tma = true;
         }
       }
-      if (dtype == SIMCLR_BF16 && out_dtype == SIMCLR_BF16) rc = dispatch_igemm<__nv_bfloat16, __nv_bfloat16>(bn, a_tma, false, false, ta, tb, tb, g, st);
-      else if (dtype == SIMCLR_BF16 && out_dtype == SIMCLR_F32) rc = dispatch_igemm<__nv_bfloat16, float>(bn, a_tma, false, false, ta, tb, tb, g, st);
-      else if (dtype == SIMCLR_F32 && out_dtype == SIMCLR_F32) rc = dispatch_igemm<float, float>(bn, a_tma, false, false, ta, tb, tb, g, st);
+      if (dtype == SIMCLR_BF16 && out_dtype == SIMCLR_BF16) rc = dispatch_igemm<__nv_bfloat16, __nv_bfloat16>(bn, a_tma, false, false, ta, tbc, tbc, g, st);
+      else if (dtype == SIMCLR_BF16 && out_dtype == SIMCLR_F32) rc = dispatch_igemm<__nv_bfloat16, float>(bn, a_tma, false, false, ta, tbc, tbc, g, st);
+      else if (dtype == SIMCLR_F32 && out_dtype == SIMCLR_F32) rc = dispatch_igemm<float, float>(bn, a_tma, false, false, ta, tbc, tbc, g, st);
       else { set_error("conv2d_dgrad_tc: unsupported dtype combination"); return SIMCLR_ERR_UNSUPPORTED; }
       if (rc) return rc;
     }
@@ -1080,26 +1208,44 @@ int run_dgrad_strided(const void* dy, const void* wd, void* dx, int dtype, int o
   return SIMCLR_OK;
 }
 
-template <typename T, int BN, bool SMALLC, bool A_TMA, bool TMA_RED>
+inline int wgrad_grid(const Geom& g) {
+  const int grid = g.tiles_m * g.tiles_n * g.splits;
+  return grid > num_sms() ? num_sms() : grid;
+}
+template <typename T, int BN, bool SMALLC, bool A_TMA, bool TMA_RED, bool MC>
 int launch_wgrad(const CUtensorMap& tx, const CUtensorMap& tdy, const CUtensorMap& tdw, const Geom& g, float* dw,
                  cudaStream_t st) {
-  auto kern = wgrad_kernel<T, BN, SMALLC, A_TMA, TMA_RED>;
+  auto kern = wgrad_kernel<T, BN, SMALLC, A_TMA, TMA_RED, MC>;
   int rc = set_smem_attr(kern, WTile<BN>::SMEM_BYTES); if (rc) return rc;      // per device: set every time
-  int grid = g.tiles_m * g.tiles_n * g.splits; if (grid > num_sms()) grid = num_sms();
-  kern<<<grid, wgrad_threads(A_TMA), WTile<BN>::SMEM_BYTES, st>>>(tx, tdy, tdw, g, dw);
-  SIMCLR_CHECK_LAUNCH();
-  return SIMCLR_OK;
+  return launch_kernel(kern, wgrad_grid(g), wgrad_threads(A_TMA), WTile<BN>::SMEM_BYTES, MC, st, tx, tdy, tdw, g, dw);
 }
 template <typename T, int BN>
 int dispatch_wgrad2(bool smallc, bool a_tma, bool tma_red, const CUtensorMap& tx, const CUtensorMap& tdy,
                     const CUtensorMap& tdw, const Geom& g, float* dw, cudaStream_t st) {
-  if (smallc) return launch_wgrad<T, BN, true, false, false>(tx, tdy, tdw, g, dw, st);
+  if (smallc) return launch_wgrad<T, BN, true, false, false, false>(tx, tdy, tdw, g, dw, st);
   if (tma_red) {
-    if (a_tma) return launch_wgrad<T, BN, false, true, true>(tx, tdy, tdw, g, dw, st);
-    return launch_wgrad<T, BN, false, false, true>(tx, tdy, tdw, g, dw, st);
+    if (a_tma && g.mc) return launch_wgrad<T, BN, false, true, true, true>(tx, tdy, tdw, g, dw, st);
+    if (a_tma) return launch_wgrad<T, BN, false, true, true, false>(tx, tdy, tdw, g, dw, st);
+    return launch_wgrad<T, BN, false, false, true, false>(tx, tdy, tdw, g, dw, st);
   }
-  if (a_tma) return launch_wgrad<T, BN, false, true, false>(tx, tdy, tdw, g, dw, st);
-  return launch_wgrad<T, BN, false, false, false>(tx, tdy, tdw, g, dw, st);
+  if (a_tma && g.mc) return launch_wgrad<T, BN, false, true, false, true>(tx, tdy, tdw, g, dw, st);
+  if (a_tma) return launch_wgrad<T, BN, false, true, false, false>(tx, tdy, tdw, g, dw, st);
+  return launch_wgrad<T, BN, false, false, false, false>(tx, tdy, tdw, g, dw, st);
+}
+
+int max_active_clusters(int size) {
+  auto kern = igemm_kernel<__nv_bfloat16, __nv_bfloat16, 128, true, false, true, true, true>;
+  if (set_smem_attr(kern, Tile<128>::SMEM_BYTES)) return 0;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(size * num_sms()); cfg.blockDim = dim3(igemm_threads(true, true));
+  cfg.dynamicSmemBytes = Tile<128>::SMEM_BYTES;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = size; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+  cfg.attrs = &attr; cfg.numAttrs = 1;
+  int n = 0;
+  if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess) { cudaGetLastError(); return 0; }
+  return n;
 }
 template <typename T>
 int dispatch_wgrad(int bn, bool smallc, bool a_tma, bool tma_red, const CUtensorMap& tx, const CUtensorMap& tdy,
@@ -1159,6 +1305,16 @@ int run_sum_partials_f64(const double* ws, int64_t stride, double* dst, int64_t 
 using namespace simclr;
 
 extern "C" {
+
+int simclr_set_tc_multicast(int on) {
+  const int prev = tc::multicast_enabled() ? 1 : 0;
+  tc::g_multicast = on ? 1 : 0;
+  return prev;
+}
+
+int simclr_tc_max_active_clusters(int size) {
+  return size > 0 ? tc::max_active_clusters(size) : 0;
+}
 
 int simclr_conv2d_fprop_tc(const void* x, const void* wf, void* y, int dtype, int y_dtype, int64_t N, int64_t H,
                            int64_t W, int64_t Cs, int64_t Cout, int64_t R, int64_t S, int64_t stride, double* bn_sums,
@@ -1262,6 +1418,9 @@ static int wgrad_tc_impl(const void* x, const void* dy, float* dw, int dtype, in
       g.im2col = 1; g.im_base = pl.lo; a_tma = true;
     }
   }
+  // the shared tile is split by 64-wide atoms: X always has two, dY two only with 128 output channels per block; a
+  // pair shares dY only inside one split (tiles_m even)
+  g.mc = a_tma ? plan_multicast(wgrad_grid(g), g.tiles_m, g.tiles_n, bn == 128 && g.tiles_m % 2 == 0) : 0;
   // splits are combined by TMA reduce-add when dW is a plain [R*S*Cin][Cout] fp32 matrix with 16-byte rows
   CUtensorMap tdw;
   const bool tma_red = !stem && Cs == Cin && aligned16(dw) && (Cout * 4) % 16 == 0;
