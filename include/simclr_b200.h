@@ -346,6 +346,14 @@ SIMCLR_API int simclr_tc_max_active_clusters(int size);
 SIMCLR_API int simclr_conv2d_fprop_tc(const void* x, const void* wf, void* y, int dtype, int y_dtype,
                                       int64_t N, int64_t H, int64_t W, int64_t Cs, int64_t Cout, int64_t R,
                                       int64_t S, int64_t stride, double* bn_sums, void* stream);
+/* Forward of a conv whose following BatchNorm coefficients are known (the replay of a recomputed block):
+ * y as simclr_conv2d_fprop_tc writes it (y_dtype = dtype = bf16) and z = act(y * scale + shift) [C = Cout],
+ * act = ReLU when relu != 0 -- the bits of simclr_conv2d_fprop_tc followed by simclr_bn_apply.  Layers on the
+ * TMA-fed implicit-GEMM kernel write z from its epilogue; the others run the conv and then the apply kernel. */
+SIMCLR_API int simclr_conv2d_fprop_tc_apply(const void* x, const void* wf, void* y, void* z, int dtype, int64_t N,
+                                            int64_t H, int64_t W, int64_t Cs, int64_t Cout, int64_t R, int64_t S,
+                                            int64_t stride, const float* scale, const float* shift, int relu,
+                                            void* stream);
 SIMCLR_API int simclr_conv2d_dgrad_tc(const void* dy, const void* wd, void* dx, int dtype, int dx_dtype,
                                       int64_t N, int64_t H, int64_t W, int64_t Cin, int64_t Cout, int64_t R,
                                       int64_t S, int64_t stride, void* stream);

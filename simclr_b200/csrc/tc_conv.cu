@@ -85,6 +85,8 @@ struct Geom {
   int im2col, im_base, im_nimg;
   int accum;           // fp32 outputs only: add into `out` (TMA reduce-add / atomics) instead of storing (tc3 passes)
   int mc;              // 2-CTA multicast: 0 off, 1 the pair shares the A (X) tile, 2 the B (dY) tile
+  // fprop with known BatchNorm coefficients (APPLY): z = act(fmaf(float(y), scale[c], shift[c])) next to y
+  void* z; const float* scale; const float* shift; int relu;
 };
 
 template <typename T> struct Elt;
@@ -182,8 +184,8 @@ __device__ __forceinline__ SmemCtl carve(uint8_t* base, int stage_bytes) {
 // ===========================================================================
 // fprop / dgrad / dense:  out[M][n_out] = gather(src)[M][K] * Wk[n_out][K]^T
 // ===========================================================================
-template <typename T, typename To, int BN, bool A_TMA, bool SMALLC, bool TMA_EPI, bool STATS, bool MC>
-__global__ void __launch_bounds__(igemm_threads(A_TMA, STATS), 1)
+template <typename T, typename To, int BN, bool A_TMA, bool SMALLC, bool TMA_EPI, bool STATS, bool MC, bool APPLY = false>
+__global__ void __launch_bounds__(igemm_threads(A_TMA, STATS || APPLY), 1)
 igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
              const __grid_constant__ CUtensorMap tmap_out, const Geom g, double* __restrict__ bn_sums) {
   using TL = Tile<BN>;
@@ -193,6 +195,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
   constexpr int CH = Elt<T>::CH;
   constexpr int NF = BN / 2;                          // accumulator registers per thread and m64 half
   static_assert(!MC || A_TMA, "multicast needs both operands fed by TMA");
+  static_assert(!APPLY || (A_TMA && TMA_EPI && !STATS && sizeof(To) == 2), "the apply epilogue is a bf16 TMA-fed fprop");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -214,8 +217,9 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
     if (TMA_EPI) tma_prefetch_desc(&tmap_out);
   }
   // With TMA-fed activations warps 5-8 have no gather to do: they take the BatchNorm statistics off the
-  // epilogue's critical path (short-K 1x1 layers are epilogue-bound).
+  // epilogue's critical path (short-K 1x1 layers are epilogue-bound), or (APPLY) write z from the staged y.
   constexpr bool STATS_WARPS = STATS && A_TMA;
+  constexpr bool AUX_WARPS = STATS_WARPS || APPLY;
   constexpr int BOX_COLS = 128 / (int)sizeof(To);     // 64 (bf16) / 32 (fp32) output columns per staged tile
   constexpr int BOXES = BN / BOX_COLS;
   constexpr int CPC = 16 / (int)sizeof(To);           // columns per 16-byte chunk: 8 (bf16) / 4 (fp32)
@@ -279,7 +283,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
           if (n0 >= g.n_out) continue;                     // uniform across the CTA
           if (threadIdx.x == 0) {
             tma_store_wait_read<1>();   // the store issued two boxes ago has read its tile
-            if (STATS_WARPS) mbar_wait(&ctl.sfree[box_ctr & 1], ((box_ctr >> 1) & 1) ^ 1);   // ... and so have the stats warps
+            if (AUX_WARPS) mbar_wait(&ctl.sfree[box_ctr & 1], ((box_ctr >> 1) & 1) ^ 1);   // ... and so have the aux warps
           }
           named_barrier_sync(1, EPI_THREADS);
           stage_frag<To>(smem_u32(stage), acc, b * BOX_COLS / 8, all_rows);
@@ -289,7 +293,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
             if (sizeof(To) == 4 && g.accum) tma_reduce_add_2d(&tmap_out, stage, n0, tm * 128);
             else tma_store_2d(&tmap_out, stage, n0, tm * 128);
             tma_store_commit();
-            if (STATS_WARPS) mbar_arrive(&ctl.sfull[box_ctr & 1]);
+            if (AUX_WARPS) mbar_arrive(&ctl.sfull[box_ctr & 1]);
           }
           if (STATS && !STATS_WARPS) {
             float a0[CPC], a1[CPC];
@@ -426,6 +430,52 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
     }
     __syncwarp();
   } else {
+    // ------------------------------ apply warps (replay fprop) -------------
+    // Each staged bf16 box [128 rows][64 columns] of y becomes z = act(fmaf(float(y), scale, shift)) -- the
+    // arithmetic and rounding of bn_apply_kernel (bn.cu) -- stored with 16-byte writes; rows >= M are skipped.
+    if (APPLY) {
+      const int ap_t = threadIdx.x - AUX_T0;
+      const int sj = ap_t & 7, srg = ap_t >> 3;
+      uint32_t ctr = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int tm = tile / g.tiles_n, tn = tile - tm * g.tiles_n;
+#pragma unroll
+        for (int b = 0; b < BOXES; ++b) {
+          const int n0 = tn * BN + b * BOX_COLS;
+          if (n0 >= g.n_out) continue;
+          const int col = n0 + sj * 8;
+          float sc[8], sh[8];
+#pragma unroll
+          for (int k = 0; k < 8; ++k) {
+            sc[k] = col < g.n_out ? __ldg(g.scale + col + k) : 0.f;
+            sh[k] = col < g.n_out ? __ldg(g.shift + col + k) : 0.f;
+          }
+          const uint8_t* stage = ctl.epi + (ctr & 1) * A_STAGE_BYTES;
+          mbar_wait(&ctl.sfull[ctr & 1], (ctr >> 1) & 1);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const long long row = (long long)tm * 128 + srg * 8 + i;
+            const uint4 raw = *reinterpret_cast<const uint4*>(stage + (srg * 8 + i) * 128 + ((sj ^ i) << 4));
+            if (row < g.M && col < g.n_out) {
+              const uint32_t w[4] = {raw.x, raw.y, raw.z, raw.w};
+              uint32_t o[4];
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                float lo = fmaf(__uint_as_float(w[e] << 16), sc[2 * e], sh[2 * e]);
+                float hi = fmaf(__uint_as_float(w[e] & 0xffff0000u), sc[2 * e + 1], sh[2 * e + 1]);
+                if (g.relu) { lo = fmaxf(lo, 0.f); hi = fmaxf(hi, 0.f); }
+                __nv_bfloat162 h2 = __floats2bfloat162_rn(lo, hi);
+                o[e] = *reinterpret_cast<uint32_t*>(&h2);
+              }
+              *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(g.z) + row * g.ldc + col) =
+                  make_uint4(o[0], o[1], o[2], o[3]);
+            }
+          }
+          warp_arrive(&ctl.sfree[ctr & 1]);
+          ++ctr;
+        }
+      }
+    }
     // ------------------------------ statistics warps (TMA-fed kernels) -----
     if (STATS_WARPS) {
       const int st_t = threadIdx.x - AUX_T0;
@@ -939,13 +989,21 @@ int launch_kernel(void (*kern)(P...), int grid, int threads, size_t smem, bool p
   return SIMCLR_OK;
 }
 
-template <typename T, typename To, int BN, bool A_TMA, bool SMALLC, bool TMA_EPI, bool STATS, bool MC>
+template <typename T, typename To, int BN, bool A_TMA, bool SMALLC, bool TMA_EPI, bool STATS, bool MC, bool APPLY = false>
 int launch_igemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout, const Geom& g, double* bn_sums,
                  cudaStream_t st) {
-  auto kern = igemm_kernel<T, To, BN, A_TMA, SMALLC, TMA_EPI, STATS, MC>;
+  auto kern = igemm_kernel<T, To, BN, A_TMA, SMALLC, TMA_EPI, STATS, MC, APPLY>;
   { int rc = set_smem_attr(kern, Tile<BN>::SMEM_BYTES); if (rc) return rc; }   // a per-DEVICE attribute: set on every launch
-  return launch_kernel(kern, igemm_grid(g, STATS), igemm_threads(A_TMA, STATS), Tile<BN>::SMEM_BYTES, MC, st, ta, tb, tout, g,
-                       bn_sums);
+  return launch_kernel(kern, igemm_grid(g, STATS), igemm_threads(A_TMA, STATS || APPLY), Tile<BN>::SMEM_BYTES, MC, st, ta, tb,
+                       tout, g, bn_sums);
+}
+
+template <int BN>
+int dispatch_igemm_apply(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout, const Geom& g,
+                         cudaStream_t st) {
+  typedef __nv_bfloat16 B;
+  if (g.mc) return launch_igemm<B, B, BN, true, false, true, false, true, true>(ta, tb, tout, g, nullptr, st);
+  return launch_igemm<B, B, BN, true, false, true, false, false, true>(ta, tb, tout, g, nullptr, st);
 }
 
 template <typename T, typename To, int BN, bool TMA_EPI, bool STATS>
@@ -1019,9 +1077,12 @@ inline StemGeom stem_geom(bool smallc, int mode, int64_t W, int64_t S, int64_t s
 
 // Shared driver for fprop (mode 0) and dgrad (mode 1).
 //   gathered tensor [N][Hs][Ws][Cs]; GEMM rows = N*P*Q; weights wk [n_out][Kp]
+// `apply` (fprop with known BatchNorm coefficients: z, scale, shift, relu of a Geom): a bf16 layer fed by TMA with a
+// TMA-store epilogue writes z in the same launch and sets *applied; any other layer writes y only.
 int run_igemm(int mode, const void* src, const void* wk, void* out, int dtype, int out_dtype, int64_t N, int64_t Hs,
               int64_t Ws, int64_t Cs, int64_t P, int64_t Q, int64_t n_out, int64_t R, int64_t S, int64_t stride,
-              cudaStream_t st, const char* what, double* bn_sums = nullptr, bool accum = false) {
+              cudaStream_t st, const char* what, double* bn_sums = nullptr, bool accum = false,
+              const Geom* apply = nullptr, int* applied = nullptr) {
   const int es = dtype == SIMCLR_BF16 ? 2 : 4;
   const int KBE = 128 / es, CH = 16 / es;
   if (accum && (out_dtype != SIMCLR_F32 || bn_sums)) { set_error("%s: accumulation needs fp32 outputs and no fused statistics", what); return SIMCLR_ERR_INVALID_ARG; }
@@ -1085,6 +1146,12 @@ int run_igemm(int mode, const void* src, const void* wk, void* out, int dtype, i
   const bool tma_epi = aligned16(out) && ((n_out * eo) % 16 == 0);
   if (tma_epi) { rc = make_tmap_2d(&tout, out, eo, (uint64_t)M, (uint64_t)n_out, (uint64_t)n_out * eo, 128, (uint32_t)(128 / eo)); if (rc) return rc; }
   else tout = tb;
+  if (apply && a_tma && tma_epi && !bn_sums && !accum && dtype == SIMCLR_BF16 && out_dtype == SIMCLR_BF16 &&
+      aligned16(apply->z)) {
+    g.z = apply->z; g.scale = apply->scale; g.shift = apply->shift; g.relu = apply->relu;
+    *applied = 1;
+    return bn == 128 ? dispatch_igemm_apply<128>(ta, tb, tout, g, st) : dispatch_igemm_apply<64>(ta, tb, tout, g, st);
+  }
   double* parts = nullptr;            // fused statistics: [CTAs][4 warps][2][n_out] partials, added in order
   const int nparts = 4 * igemm_grid(g, true);
   if (bn_sums) {
@@ -1325,6 +1392,24 @@ int simclr_conv2d_fprop_tc(const void* x, const void* wf, void* y, int dtype, in
   const int64_t Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
   return tc::run_igemm(0, x, wf, y, dtype, y_dtype, N, H, W, Cs, Ho, Wo, Cout, R, S, stride, (cudaStream_t)stream,
                        "conv2d_fprop_tc", bn_sums);
+}
+
+int simclr_conv2d_fprop_tc_apply(const void* x, const void* wf, void* y, void* z, int dtype, int64_t N, int64_t H,
+                                 int64_t W, int64_t Cs, int64_t Cout, int64_t R, int64_t S, int64_t stride,
+                                 const float* scale, const float* shift, int relu, void* stream) {
+  SIMCLR_CHECK_ARG(x && wf && y && z && scale && shift, "conv2d_fprop_tc_apply: null pointer");
+  SIMCLR_CHECK_ARG(dtype == SIMCLR_BF16, "conv2d_fprop_tc_apply: bf16 activations only");
+  SIMCLR_CHECK_ARG(N > 0 && H > 0 && W > 0 && Cs > 0 && Cout > 0 && Cout % 8 == 0 && R > 0 && S > 0 && (R & 1) && (S & 1) &&
+                   stride > 0, "conv2d_fprop_tc_apply: bad geometry");
+  const int64_t Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
+  tc::Geom ap;
+  ap.z = z; ap.scale = scale; ap.shift = shift; ap.relu = relu ? 1 : 0;
+  int applied = 0;
+  int rc = tc::run_igemm(0, x, wf, y, dtype, dtype, N, H, W, Cs, Ho, Wo, Cout, R, S, stride, (cudaStream_t)stream,
+                         "conv2d_fprop_tc_apply", nullptr, false, &ap, &applied);
+  if (rc || applied) return rc;
+  // the halo 3x3, stem and gathered layers: conv, then the BatchNorm apply kernel
+  return simclr_bn_apply(y, dtype, nullptr, z, dtype, N * Ho * Wo, Cout, scale, shift, relu, stream);
 }
 
 int simclr_conv2d_dgrad_tc(const void* dy, const void* wd, void* dx, int dtype, int dx_dtype, int64_t N, int64_t H,

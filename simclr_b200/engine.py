@@ -188,6 +188,10 @@ class Engine:
         self._pack_ops = []
         self._pack_table = None
         self.pack_token = None
+        # activation recomputation (resnet.BlockGroup): 'record' while a recomputed block group runs its training
+        # forward (its BatchNorms keep their coefficients), 'replay' while a block re-runs that forward in the
+        # backward pass (BatchNorms apply the kept coefficients: no statistics, exchange or moving-average update)
+        self.recompute = None
 
     # -- helpers ---------------------------------------------------------
     def code(self, dtype):
@@ -229,6 +233,11 @@ class Engine:
         t = self._sums_pool[self._sums_cursor:self._sums_cursor + n]
         self._sums_cursor += n_al
         return t
+
+    def bn_sums(self, n):
+        """`sums(n)` for the statistics a conv epilogue produces in a training forward; None in a replay, which
+        applies kept BatchNorm coefficients and takes no statistics."""
+        return None if self.recompute == 'replay' else self.sums(n)
 
     # -- packed tensor-core operands -------------------------------------------------
     def register_packed(self, op):

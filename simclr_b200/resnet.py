@@ -34,10 +34,22 @@ class BatchNormRelu:  # pylint: disable=missing-docstring
         self.moving_mean = vs.add(pre + '/moving_mean:0', (channels,), 'zeros', trainable=False)
         self.moving_variance = vs.add(pre + '/moving_variance:0', (channels,), 'ones', trainable=False)
         self.saved = None
+        self.kept = None       # (mean, rstd, scale, shift) of the last training forward of a recomputed block
 
     def _statistics(self, y, training, sums=None):
         """(mean, rstd, scale, shift) of this call: batch statistics (SyncBN: global, exchanged over peer memory or
-        NCCL) with the moving-average update when training, the moving statistics otherwise."""
+        NCCL) with the moving-average update when training, the moving statistics otherwise.  In a recomputed
+        block the training forward keeps them and the replay in the backward pass reuses them, so the replay
+        produces the same bits without taking statistics, exchanging them or updating the moving averages."""
+        e = get_engine()
+        if training and e.recompute == 'replay':
+            return self.kept
+        stats = self._compute_statistics(y, training, sums)
+        if training and e.recompute == 'record':
+            self.kept = stats
+        return stats
+
+    def _compute_statistics(self, y, training, sums):
         e = get_engine()
         C = self.C
         rows = y.numel() // C
@@ -185,6 +197,14 @@ class BatchNormRelu:  # pylint: disable=missing-docstring
             self.saved = (y, bits, mean, rstd, rows, (scale, shift) if (relu and residual is None) else None)
         return z
 
+    def replay_apply(self, op, x):
+        """Replay of conv `op` -> this BatchNorm(+ReLU) without a residual: the conv epilogue applies the kept
+        coefficients, so y and z come from one launch with the bits of `op.forward` followed by `__call__`."""
+        mean, rstd, scale, shift = self.kept
+        y, z = op.forward_apply(x, scale, shift, self.relu)
+        self.saved = (y, None, mean, rstd, y.numel() // self.C, (scale, shift) if self.relu else None)
+        return z
+
     def backward(self, dz, dz2=None, dy_dtype=None):
         """dz (and dz2) are gradients w.r.t. the layer output.  For the block tail
         (residual add + ReLU) dz is overwritten with (dz + dz2) * relu_mask, which the
@@ -291,13 +311,16 @@ class ConvOp:
         Ho, Wo = (H - 1) // s + 1, (W - 1) // s + 1
         y = e.empty((N, Ho, Wo, self.cout), out_dtype or e.act_dtype)
         st = stream_ptr()
+        replay = e.recompute == 'replay'          # the packed operands are this step's: its forward made them
         if e.conv_engine == 'tc':
-            self._pack(e)
+            if not replay:
+                self._pack(e)
             self._timed(e, 'fprop', x.shape, lambda: lib.conv2d_fprop_tc(
                 x, self.wf, y, e.code(x.dtype), e.code(y.dtype), N, H, W, Cs, self.cout, self.R, self.S, s, bn_sums, st))
         elif e.conv_engine == 'tc3':
             assert x.dtype == torch.float32 and y.dtype == torch.float32, 'tc3 (split bf16) is the fp32-storage mode'
-            self._pack3(e)
+            if not replay:
+                self._pack3(e)
             xs = self._split(e, x)
             self._timed(e, 'fprop', x.shape, lambda: lib.conv2d_fprop_tc3(
                 xs[0], xs[1], xs[2], self.wf3[0], self.wf3[1], self.wf3[2], y, N, H, W, Cs, self.cout, self.R, self.S, s, st))
@@ -314,6 +337,22 @@ class ConvOp:
         if training:
             self.saved_x = x
         return y
+
+    def forward_apply(self, x, scale, shift, relu):
+        """Training forward of a bf16 tensor-core conv whose BatchNorm coefficients are already known (a replay):
+        returns y and z = act(y * scale + shift), both written by the conv's epilogue."""
+        e = get_engine()
+        N, H, W, Cs = x.shape
+        assert Cs == self.cs, (x.shape, self.cs)
+        s = self.stride
+        Ho, Wo = (H - 1) // s + 1, (W - 1) // s + 1
+        y = e.empty((N, Ho, Wo, self.cout), x.dtype)
+        z = e.empty(y.shape, x.dtype)
+        self._timed(e, 'fprop', x.shape, lambda: lib.conv2d_fprop_tc_apply(
+            x, self.wf, y, z, e.code(x.dtype), N, H, W, Cs, self.cout, self.R, self.S, s, scale, shift, int(relu),
+            stream_ptr()))
+        self.saved_x = x
+        return y, z
 
     def backward(self, dy, need_dx=True, dx_dtype=None):
         e = get_engine()
@@ -388,7 +427,9 @@ def conv_bn(conv, bn, x, training, **bn_kwargs):
     op = conv.op if hasattr(conv, 'op') else conv
     if not training:
         return bn(op.forward(x, training), training, **bn_kwargs)
-    sums = e.sums(2 * op.cout)
+    if e.recompute == 'replay' and not bn_kwargs and e.conv_engine == 'tc' and x.dtype == torch.bfloat16:
+        return bn.replay_apply(op, x)
+    sums = e.bn_sums(2 * op.cout)
     y = op.forward(x, training, bn_sums=sums)
     return bn(y, training, sums=sums, **bn_kwargs)
 
@@ -443,7 +484,7 @@ class _Shortcut:
         """Training only: the conv output and its batch statistics; the BatchNorm is applied by the block tail
         (`BatchNormRelu.forward_tail2`)."""
         e = get_engine()
-        sums = e.sums(2 * self.conv.cout)
+        sums = e.bn_sums(2 * self.conv.cout)
         return self.conv.op.forward(self._pre(x), True, bn_sums=sums), sums
 
     def backward(self, d):
@@ -616,7 +657,40 @@ class _AddRelu:
         return d_out
 
 
-class ResidualBlock:  # pylint: disable=missing-docstring
+def _drop_saved(layer):
+    """Releases everything `layer` and its sub-layers keep for their backward pass (BatchNorm `kept`
+    coefficients stay)."""
+    for k, v in vars(layer).items():
+        if k in ('saved', 'saved_x'):
+            setattr(layer, k, None)
+        elif isinstance(v, (BatchNormRelu, ConvOp, Conv2dFixedPadding, _Shortcut, SK_Conv2D, SE_Layer, _AddRelu)):
+            _drop_saved(v)
+
+
+class _Recomputed:
+    """Activation recomputation of a residual block.  After a training forward run with the engine in 'record'
+    mode the block keeps only a reference to its input (the previous block's output, stored anyway) and its
+    BatchNorms' coefficients; `replay` re-runs that forward before the block's backward pass.  The step is
+    deterministic and the replay applies the kept coefficients, so every tensor it re-creates has the bits the
+    first forward produced."""
+
+    replay_input = None
+
+    def release(self, inputs):
+        self.replay_input = inputs
+        _drop_saved(self)
+
+    def replay(self):
+        e = get_engine()
+        e.recompute = 'replay'
+        try:
+            self(self.replay_input, True)
+        finally:
+            e.recompute = None
+        self.replay_input = None
+
+
+class ResidualBlock(_Recomputed):  # pylint: disable=missing-docstring
     """tf2/resnet.py:314-382."""
 
     def __init__(self, vs, scope, cin, filters, strides, use_projection=False):
@@ -642,7 +716,7 @@ class ResidualBlock:  # pylint: disable=missing-docstring
             x = self.se_layer(conv_bn(self.c2, self.b2, x, training), training)
             return self.add_relu(x, shortcut, training)
         if self.fused_tail:
-            sums = get_engine().sums(2 * self.c2.cout)
+            sums = get_engine().bn_sums(2 * self.c2.cout)
             return self.b2.forward_tail2(self.c2.op.forward(x, True, bn_sums=sums), sums, ys, self.shortcut.bn, sums_s)
         return conv_bn(self.c2, self.b2, x, training, residual=shortcut, relu=True)     # relu(inputs + shortcut), :382
 
@@ -665,7 +739,7 @@ class ResidualBlock:  # pylint: disable=missing-docstring
         return dx_a, dx_b
 
 
-class BottleneckBlock:
+class BottleneckBlock(_Recomputed):
     """tf2/resnet.py:385-487 (DropBlock is dead code in the reference, SURVEY Q2)."""
 
     def __init__(self, vs, scope, cin, filters, strides, use_projection=False):
@@ -699,7 +773,7 @@ class BottleneckBlock:
             x = self.se_layer(conv_bn(self.c3, self.b3, x, training), training)
             return self.add_relu(x, shortcut, training)
         if self.fused_tail:
-            sums = get_engine().sums(2 * self.c3.cout)
+            sums = get_engine().bn_sums(2 * self.c3.cout)
             return self.b3.forward_tail2(self.c3.op.forward(x, True, bn_sums=sums), sums, ys, self.shortcut.bn, sums_s)
         return conv_bn(self.c3, self.b3, x, training, residual=shortcut, relu=True)     # relu(inputs + shortcut), :487
 
@@ -737,14 +811,28 @@ class BlockGroup:  # pylint: disable=missing-docstring
         for _ in range(1, blocks):
             self.layers.append(block_fn(vs, scope, self.layers[-1].cout, filters, 1))
         self.cout = self.layers[-1].cout
+        self.recompute = False       # keep only the block outputs; replay each block in the backward pass
 
     def __call__(self, inputs, training):
-        for layer in self.layers:
-            inputs = layer(inputs, training)
+        if not (training and self.recompute):
+            for layer in self.layers:
+                inputs = layer(inputs, training)
+            return inputs
+        e = get_engine()
+        e.recompute = 'record'
+        try:
+            for layer in self.layers:
+                out = layer(inputs, True)
+                layer.release(inputs)
+                inputs = out
+        finally:
+            e.recompute = None
         return inputs
 
     def backward(self, d, d2=None):
         for layer in reversed(self.layers):
+            if layer.replay_input is not None:
+                layer.replay()
             d, d2 = layer.backward(d, d2)
         return d, d2
 
@@ -755,7 +843,7 @@ class Resnet:  # pylint: disable=missing-docstring
 
     STEM_CS = 4
 
-    def __init__(self, vs, block_fn, layers, width_multiplier, cifar_stem=False):
+    def __init__(self, vs, block_fn, layers, width_multiplier, cifar_stem=False, recompute=()):
         scope = 'resnet'
         wm = width_multiplier
         self.cifar_stem = cifar_stem
@@ -792,6 +880,21 @@ class Resnet:  # pylint: disable=missing-docstring
         vs.default_trainable = True
         self.cout = cin
         self.saved = None
+        self.recompute = recompute
+
+    @property
+    def recompute(self):
+        """Block groups (1-4) whose activations are recomputed in the backward pass.  Frozen groups of a
+        finetuning run store nothing and are never recomputed."""
+        return frozenset(i + 1 for i, g in enumerate(self.block_groups) if g.recompute)
+
+    @recompute.setter
+    def recompute(self, groups):
+        groups = frozenset(groups or ())
+        if not groups <= {1, 2, 3, 4}:
+            raise ValueError('recompute: block groups are 1-4, got %s' % sorted(groups))
+        for i, g in enumerate(self.block_groups):
+            g.recompute = (i + 1) in groups and not (self.stem_frozen and i < self.frozen_groups)
 
     def __call__(self, inputs, training, endpoints=None):
         e = get_engine()
@@ -899,12 +1002,13 @@ MODEL_PARAMS = {  # tf2/resnet.py:709-734
 
 
 def resnet(resnet_depth, width_multiplier, cifar_stem=False, data_format='channels_last',
-           dropblock_keep_probs=None, dropblock_size=None, vs=None):
+           dropblock_keep_probs=None, dropblock_size=None, vs=None, recompute=()):
     """Returns the ResNet model for a given size (tf2/resnet.py:702-747, same arguments).
 
     `vs` (this implementation only): the `engine.VarStore` the variables are registered in; a
     fresh one is created when omitted (exposed as `.vs`, call `.vs.materialize(device)` before
-    use).  Only `channels_last` exists on this path."""
+    use).  Only `channels_last` exists on this path.  `recompute`: the block groups (1-4) whose activations are
+    recomputed in the backward pass (`Resnet.recompute`)."""
     from .engine import VarStore
     if resnet_depth not in MODEL_PARAMS:
         raise ValueError('Not a valid resnet_depth:', resnet_depth)
@@ -914,6 +1018,6 @@ def resnet(resnet_depth, width_multiplier, cifar_stem=False, data_format='channe
     block_fn, layers = MODEL_PARAMS[resnet_depth]
     if vs is None:
         vs = VarStore()
-    net = Resnet(vs, block_fn, layers, width_multiplier, cifar_stem=cifar_stem)
+    net = Resnet(vs, block_fn, layers, width_multiplier, cifar_stem=cifar_stem, recompute=recompute)
     net.vs = vs
     return net

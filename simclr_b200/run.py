@@ -28,9 +28,13 @@ from .comm import gather_fits
 class Trainer:
     """Owns model + optimizer and runs `single_step` (tf2/run.py:557-622)."""
 
-    def __init__(self, num_classes=None, num_examples=None, seed=0, engine=None, teacher=None):
+    def __init__(self, num_classes=None, num_examples=None, seed=0, engine=None, teacher=None, recompute=None):
         """`teacher` (a `distill.Teacher`, finetune mode only): the training loss becomes SimCLRv2 distillation on
-        the teacher's logits, and the student's class count is the teacher's."""
+        the teacher's logits, and the student's class count is the teacher's.
+
+        `recompute`: block groups (1-4) whose activations are recomputed in the backward pass.  None chooses them
+        from the byte model of `memory.py` (the fewest groups that make the step fit the card; none when it fits
+        as it is); SIMCLR_RECOMPUTE=off / all overrides that choice."""
         self.engine = engine or engine_lib.get_engine()
         self.strategy = self.engine.ctx
         self.teacher = teacher
@@ -48,6 +52,7 @@ class Trainer:
         self.num_classes = num_classes or FLAGS.b200_num_classes
         self.num_examples = num_examples or FLAGS.b200_num_examples
         self.model = model_lib.Model(self.num_classes, seed=seed)
+        self.model.resnet_model.recompute = self._recompute_plan() if recompute is None else recompute
         self._gcl_step = None
         if self.gcl is not None:
             obj_lib.check_generalized_contrastive(self.gcl, self._proj_dim(), 2 * FLAGS.train_batch_size)
@@ -63,6 +68,28 @@ class Trainer:
         self._split_off = None
         self._side = None
         self._top_work = None
+
+    def _recompute_plan(self):
+        from . import memory
+        mode = os.environ.get('SIMCLR_RECOMPUTE', 'auto')
+        if mode not in ('auto', 'off', 'all'):
+            raise ValueError('SIMCLR_RECOMPUTE must be auto, off or all (got %r)' % mode)
+        if mode != 'auto':
+            return {1, 2, 3, 4} if mode == 'all' else set()
+        R = self.strategy.num_replicas_in_sync
+        batch = max(FLAGS.train_batch_size // R, 1)
+        m = memory.model_from_flags(FLAGS, batch)
+        total = torch.cuda.get_device_properties(self.engine.device).total_memory
+        chosen = memory.plan(m, total)
+        if chosen:
+            logging.info('Recomputing the activations of block groups %s: predicted peak %.1f GiB of %.1f GiB '
+                         '(%.1f GiB without recomputation)', memory.describe(chosen),
+                         memory.gib(memory.predicted_peak(m, chosen)), memory.gib(total),
+                         memory.gib(memory.predicted_peak(m, set())))
+        else:
+            logging.info('No activation recomputation: predicted peak %.1f GiB of %.1f GiB',
+                         memory.gib(memory.predicted_peak(m, set())), memory.gib(total))
+        return chosen
 
     # ------------------------------------------------------------------
     GRAD_SPLIT = 2      # backward_top covers block groups 3-4 + heads: 96 % of the ResNet-50 gradient bytes
