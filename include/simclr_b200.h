@@ -328,6 +328,13 @@ SIMCLR_API int simclr_pack_conv_weight(const float* w_hwio, void* wf, void* wd, 
  * `table_dev` is a device array of n_layers rows of 10 int64 {w_hwio, wf, wd (0: none), R, S, Cin, Cs,
  * Cout, Kp, Kdp}, same layouts as simclr_pack_conv_weight with dtype bf16. */
 SIMCLR_API int simclr_pack_conv_weights_multi(const void* table_dev, int64_t n_layers, void* stream);
+/* Inference-mode BatchNorm folded into the conv / dense weights before it, for every layer in ONE launch.
+ * `table_dev`: a device array of n_layers rows of 11 int64 {w_hwio, scale, shift, wf, bias, R, S, Cin, Cs, Cout,
+ * Kp}: fp32 HWIO master, the BatchNorm's fp32 inference coefficients scale[Cout] and shift[Cout] (z = y*scale +
+ * shift on the moving statistics), and the outputs wf [Cout][Kp] bf16 in the layout of simclr_pack_conv_weight
+ * (the stem's S+1 slots included) holding bf16_rn(w * scale[co]) with the product in fp32, and bias [Cout] fp32
+ * = shift.  No dgrad copy.  Input of simclr_conv2d_fprop_tc_bias. */
+SIMCLR_API int simclr_fold_conv_bn_multi(const void* table_dev, int64_t n_layers, void* stream);
 /* Accumulation outputs -- the BatchNorm sums of simclr_conv2d_fprop_tc / simclr_bn_stats /
  * simclr_bn_bwd_*reduce and dW of simclr_conv2d_wgrad_tc -- are zeroed by the call that fills them.  A caller
  * that keeps them in pooled buffers and zeroes those once per step (simclr_memset_zero) switches the per-call
@@ -354,6 +361,18 @@ SIMCLR_API int simclr_conv2d_fprop_tc_apply(const void* x, const void* wf, void*
                                             int64_t H, int64_t W, int64_t Cs, int64_t Cout, int64_t R, int64_t S,
                                             int64_t stride, const float* scale, const float* shift, int relu,
                                             void* stream);
+/* Inference forward of conv -> BatchNorm [-> residual add] [-> ReLU] on folded weights (simclr_fold_conv_bn_multi),
+ * one launch, no y and no statistics.  x [N][H][W][Cs] bf16, wf the folded [Cout][Kp] bf16, bias [Cout] fp32,
+ * residual (nullable) [N][Ho][Wo][Cout] bf16, z [N][Ho][Wo][Cout] of z_dtype: bf16, or fp32 for a dense layer
+ * (H = W = R = S = 1).  Every output element is, in this order and in fp32 arithmetic on the fp32 accumulator:
+ *   v = acc + bias[c];  v += float(residual[row][c]) if residual;  v = max(v, 0) if relu;  z = bf16_rn(v) (fp32: v).
+ * The same epilogue runs in every fprop kernel a layer can land on: the implicit GEMM (TMA tile, TMA im2col and
+ * gathered feeds; TMA-store and direct-store epilogues), the 64/128-channel 3x3 halo kernel and the 7x7 stem
+ * kernel (no residual).  A residual needs Cout % 8 == 0. */
+SIMCLR_API int simclr_conv2d_fprop_tc_bias(const void* x, const void* wf, const float* bias, const void* residual,
+                                           void* z, int z_dtype, int64_t N, int64_t H, int64_t W, int64_t Cs,
+                                           int64_t Cout, int64_t R, int64_t S, int64_t stride, int relu,
+                                           void* stream);
 SIMCLR_API int simclr_conv2d_dgrad_tc(const void* dy, const void* wd, void* dx, int dtype, int dx_dtype,
                                       int64_t N, int64_t H, int64_t W, int64_t Cin, int64_t Cout, int64_t R,
                                       int64_t S, int64_t stride, void* stream);

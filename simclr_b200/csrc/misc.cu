@@ -261,6 +261,68 @@ __global__ void pack_weight_kernel(const float* __restrict__ w, T* __restrict__ 
   }
 }
 
+// ---- folded BatchNorm weights ------------------------------------------------
+// Table rows {w_hwio, scale, shift, wf, bias, R, S, Cin, Cs, Cout, Kp}: wf = bf16_rn(w * scale[co]) (fp32 product) in
+// the layout of pack_weight_kernel, bias = shift.  As in pack_weights_multi_kernel, 32x32 (k, co) tiles of all layers
+// are dealt round-robin over the blocks of one launch and transposed through shared memory, so that both the reads
+// of the HWIO masters (co fastest) and the writes of the K-major operands (k fastest) are coalesced.
+constexpr int FOLD_COLS = 11;
+__device__ __forceinline__ float fold_master(const float* __restrict__ w, int k, int co, int R, int S, int Cin, int Cs,
+                                             int Cout) {
+  const int tap = k / Cs, c = k % Cs;
+  if (Cs == 4) {                               // the stem's S+1 slots per filter row, slot 0 zero
+    const int r = tap / (S + 1), sp = tap % (S + 1);
+    return (r < R && sp >= 1 && c < Cin) ? w[((int64_t)(r * S + sp - 1) * Cin + c) * Cout + co] : 0.f;
+  }
+  return (tap < R * S && c < Cin) ? w[((int64_t)tap * Cin + c) * Cout + co] : 0.f;
+}
+__global__ void __launch_bounds__(256) fold_conv_bn_multi_kernel(const long long* __restrict__ table, int n_layers) {
+  __shared__ long long ustart[PACK_MAX_LAYERS + 1];
+  __shared__ float tile[32][33];
+  for (int l = threadIdx.x; l < n_layers; l += blockDim.x) {
+    const long long* t = table + (long long)l * FOLD_COLS;
+    ustart[l + 1] = ((t[10] + 31) / 32) * ((t[9] + 31) / 32);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    ustart[0] = 0;
+    for (int l = 0; l < n_layers; ++l) ustart[l + 1] += ustart[l];
+  }
+  __syncthreads();
+  const long long total = ustart[n_layers];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  for (long long u = blockIdx.x; u < total; u += gridDim.x) {
+    int lo = 0, hi = n_layers;
+    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (ustart[mid] <= u) lo = mid; else hi = mid; }
+    const long long* t = table + (long long)lo * FOLD_COLS;
+    const float* __restrict__ w = reinterpret_cast<const float*>(t[0]);
+    const float* __restrict__ scale = reinterpret_cast<const float*>(t[1]);
+    const float* __restrict__ shift = reinterpret_cast<const float*>(t[2]);
+    __nv_bfloat16* __restrict__ wf = reinterpret_cast<__nv_bfloat16*>(t[3]);
+    float* __restrict__ bias = reinterpret_cast<float*>(t[4]);
+    const int R = (int)t[5], S = (int)t[6], Cin = (int)t[7], Cs = (int)t[8], Cout = (int)t[9], Kp = (int)t[10];
+    const long long local = u - ustart[lo], tiles_k = (Kp + 31) / 32;
+    const int k0 = (int)(local % tiles_k) * 32, c0 = (int)(local / tiles_k) * 32;
+    {
+      const int co = c0 + tx;
+      const float sc = co < Cout ? __ldg(scale + co) : 0.f;
+      if (k0 == 0 && ty == 0 && co < Cout) bias[co] = shift[co];
+#pragma unroll
+      for (int r = ty; r < 32; r += 8) {
+        const int k = k0 + r;
+        tile[r][tx] = (k < Kp && co < Cout) ? fold_master(w, k, co, R, S, Cin, Cs, Cout) * sc : 0.f;
+      }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int r = ty; r < 32; r += 8) {
+      const int co = c0 + r, k = k0 + tx;
+      if (co < Cout && k < Kp) wf[(int64_t)co * Kp + k] = __float2bfloat16_rn(tile[tx][r]);
+    }
+    __syncthreads();
+  }
+}
+
 // ---- input prep ------------------------------------------------------------
 constexpr int MAX_TAPS = 65;
 // outputs per thread along the blurred axis: (2*radius + OUT) / OUT loads per output.  The vertical pass gains from 8,
@@ -514,6 +576,13 @@ int simclr_pack_conv_weight(const float* w_hwio, void* wf, void* wd, int dtype, 
 int simclr_pack_conv_weights_multi(const void* table_dev, int64_t n_layers, void* stream) {
   SIMCLR_CHECK_ARG(table_dev && n_layers > 0 && n_layers <= PACK_MAX_LAYERS, "pack_conv_weights_multi: 1..%d layers", PACK_MAX_LAYERS);
   pack_weights_multi_kernel<<<(unsigned)(num_sms() * 8), 256, 0, (cudaStream_t)stream>>>((const long long*)table_dev, (int)n_layers);
+  SIMCLR_CHECK_LAUNCH();
+  return SIMCLR_OK;
+}
+
+int simclr_fold_conv_bn_multi(const void* table_dev, int64_t n_layers, void* stream) {
+  SIMCLR_CHECK_ARG(table_dev && n_layers > 0 && n_layers <= PACK_MAX_LAYERS, "fold_conv_bn_multi: 1..%d layers", PACK_MAX_LAYERS);
+  fold_conv_bn_multi_kernel<<<(unsigned)(num_sms() * 8), 256, 0, (cudaStream_t)stream>>>((const long long*)table_dev, (int)n_layers);
   SIMCLR_CHECK_LAUNCH();
   return SIMCLR_OK;
 }

@@ -335,6 +335,66 @@ __device__ __forceinline__ void stage_frag(uint32_t tile, const float (&acc)[2][
       }
     }
 }
+// Folded BatchNorm epilogue (simclr_conv2d_fprop_tc_bias): the BatchNorm is in the packed weights and `bias`, and
+// before a tile's accumulators are rounded and stored each one becomes, in this order and in fp32,
+//   v = acc + bias[c];  v += float(res[row][c]) if res;  v = max(v, 0) if relu.
+// Registers 4*i + 2*rp + j of half h hold tile row frag_row(h, rp) and column col0 + 8*i + 2*(lane & 3) + j;
+// roff[h][rp] is that row's element offset into res (< 0: the row does not exist).  res needs an even n_out.
+// The consumer warpgroup runs this between its last MMA and the staging of the tile, with no other warp to hide a
+// load's latency: the loads of a chunk of up to 64 columns are all issued before any is used (one round trip per
+// chunk), and fold_prefetch has pulled the tile's residual rows into L2 while the MMAs ran.
+struct FoldArgs { const float* bias; const __nv_bfloat16* res; int relu; };
+template <int NF>
+__device__ __forceinline__ void fold_epilogue(float (&acc)[2][NF], const FoldArgs& f, int col0, int n_out,
+                                              const long long (&roff)[2][2]) {
+  constexpr int NI = NF / 4;                   // 8-column groups of the tile
+  constexpr int CI = NI < 8 ? NI : 8;          // groups per chunk
+  const int q = threadIdx.x & 3;
+  const bool has_res = f.res != nullptr;
+#pragma unroll
+  for (int i0 = 0; i0 < NI; i0 += CI) {
+    float b0[CI], b1[CI];
+    uint32_t rv[CI][2][2];
+#pragma unroll
+    for (int ii = 0; ii < CI; ++ii) {
+      const int c = col0 + 8 * (i0 + ii) + 2 * q;
+      b0[ii] = c < n_out ? __ldg(f.bias + c) : 0.f;
+      b1[ii] = c + 1 < n_out ? __ldg(f.bias + c + 1) : 0.f;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int rp = 0; rp < 2; ++rp)
+          rv[ii][h][rp] = has_res && roff[h][rp] >= 0 && c < n_out
+                              ? __ldg(reinterpret_cast<const unsigned int*>(f.res + roff[h][rp] + c)) : 0u;
+    }
+#pragma unroll
+    for (int ii = 0; ii < CI; ++ii)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int rp = 0; rp < 2; ++rp) {
+          const int i = i0 + ii;
+          float v0 = acc[h][4 * i + 2 * rp] + b0[ii], v1 = acc[h][4 * i + 2 * rp + 1] + b1[ii];
+          if (has_res) { v0 += __uint_as_float(rv[ii][h][rp] << 16); v1 += __uint_as_float(rv[ii][h][rp] & 0xffff0000u); }
+          if (f.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+          acc[h][4 * i + 2 * rp] = v0; acc[h][4 * i + 2 * rp + 1] = v1;
+        }
+  }
+}
+// Issued at the start of a tile, before its MMAs: the 128-byte lines of the thread's residual rows that the tile's
+// BN columns cover go to L2, so that fold_epilogue's loads after the MMAs do not wait on HBM.
+template <int BN>
+__device__ __forceinline__ void fold_prefetch(const FoldArgs& f, int col0, int n_out, const long long (&roff)[2][2]) {
+  const int q = threadIdx.x & 3;
+  const int c = col0 + q * 64;                 // 64 bf16 = one 128-byte line
+  if (f.res == nullptr || q >= BN / 64 || c >= n_out) return;
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int rp = 0; rp < 2; ++rp)
+      if (roff[h][rp] >= 0) asm volatile("prefetch.global.L2 [%0];" ::"l"(f.res + roff[h][rp] + c));
+}
+
 // the 32 fp32 values of `row` from a [128 rows][128 B] 128B-swizzled staging tile
 __device__ __forceinline__ void load_row32(const uint8_t* tile, int row, uint32_t* r) {
 #pragma unroll
@@ -446,8 +506,9 @@ inline int make_tmap_im2col(CUtensorMap* map, const void* base, int elt_bytes, u
 // 7x7 stride-2 stem fprop from a slab of 16-byte pixel pairs, no im2col copy (tc_stem.cu)
 bool stem7x7_applicable(int dtype, int out_dtype, int64_t N, int64_t H, int64_t W, int64_t Cs, int64_t n_out, int64_t R,
                         int64_t S, int64_t stride, int64_t P, int64_t Q, const void* src, const void* wk, const void* out);
+// fold (nullable, no residual): the folded epilogue writes z instead of y
 int run_stem7x7(const void* src, const void* wk, void* out, int64_t N, int64_t H, int64_t W, int64_t n_out, cudaStream_t st,
-                double* bn_sums);
+                double* bn_sums, const FoldArgs* fold = nullptr);
 bool stem7x7_wgrad_applicable(int dtype, int64_t N, int64_t H, int64_t W, int64_t Cs, int64_t Cin, int64_t Cout, int64_t R,
                               int64_t S, int64_t stride, const void* x, const void* dy, const void* dw);
 int run_stem7x7_wgrad(const void* x, const void* dy, float* dw, int64_t N, int64_t H, int64_t W, int64_t Cin, cudaStream_t st,
@@ -456,7 +517,7 @@ int run_stem7x7_wgrad(const void* x, const void* dy, float* dw, int64_t N, int64
 bool halo3x3_applicable(int dtype, int out_dtype, int64_t N, int64_t H, int64_t W, int64_t C, int64_t n_out, int64_t R,
                         int64_t S, int64_t stride, const void* src, const void* wk, const void* out);
 int run_halo3x3(int mode, const void* src, const void* wk, void* out, int64_t N, int64_t H, int64_t W, int64_t C,
-                int64_t n_out, cudaStream_t st, double* bn_sums);
+                int64_t n_out, cudaStream_t st, double* bn_sums, const FoldArgs* fold = nullptr);
 // wgrad of the 64 -> 64 channel 3x3 stride-1 layers with halo reuse (tc_halo.cu)
 bool halo3x3_wgrad_applicable(int dtype, int64_t N, int64_t H, int64_t W, int64_t Cs, int64_t Cin, int64_t Cout, int64_t R,
                               int64_t S, int64_t stride, const void* x, const void* dy, const void* dw);

@@ -87,6 +87,8 @@ struct Geom {
   int mc;              // 2-CTA multicast: 0 off, 1 the pair shares the A (X) tile, 2 the B (dY) tile
   // fprop with known BatchNorm coefficients (APPLY): z = act(fmaf(float(y), scale[c], shift[c])) next to y
   void* z; const float* scale; const float* shift; int relu;
+  // folded BatchNorm (FOLD): bias, optional residual and ReLU applied to the accumulators (fold_epilogue)
+  FoldArgs fold;
 };
 
 template <typename T> struct Elt;
@@ -184,7 +186,8 @@ __device__ __forceinline__ SmemCtl carve(uint8_t* base, int stage_bytes) {
 // ===========================================================================
 // fprop / dgrad / dense:  out[M][n_out] = gather(src)[M][K] * Wk[n_out][K]^T
 // ===========================================================================
-template <typename T, typename To, int BN, bool A_TMA, bool SMALLC, bool TMA_EPI, bool STATS, bool MC, bool APPLY = false>
+template <typename T, typename To, int BN, bool A_TMA, bool SMALLC, bool TMA_EPI, bool STATS, bool MC, bool APPLY = false,
+          bool FOLD = false>
 __global__ void __launch_bounds__(igemm_threads(A_TMA, STATS || APPLY), 1)
 igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
              const __grid_constant__ CUtensorMap tmap_out, const Geom g, double* __restrict__ bn_sums) {
@@ -196,6 +199,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
   constexpr int NF = BN / 2;                          // accumulator registers per thread and m64 half
   static_assert(!MC || A_TMA, "multicast needs both operands fed by TMA");
   static_assert(!APPLY || (A_TMA && TMA_EPI && !STATS && sizeof(To) == 2), "the apply epilogue is a bf16 TMA-fed fprop");
+  static_assert(!FOLD || (!STATS && !APPLY && !MC && !TF32), "the folded epilogue is a bf16 inference fprop");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -253,6 +257,17 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int tm = tile / g.tiles_n, tn = tile - tm * g.tiles_n;
       const bool paired = MC && tile - (int)rank + 1 < num_tiles;   // the same value on both CTAs of the pair
+      long long roff[2][2];                                           // FOLD: the thread's residual rows
+      if (FOLD) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int rp = 0; rp < 2; ++rp) {
+            const long long m = (long long)tm * 128 + frag_row(h, rp);
+            roff[h][rp] = m < g.M ? m * g.ldc : -1;
+          }
+        fold_prefetch<BN>(g.fold, tn * BN, g.n_out, roff);
+      }
       int prev = 0;
       for (int kb = 0; kb < g.num_kb; ++kb) {
         mbar_wait(&ctl.full[pp.stage], pp.phase);
@@ -272,6 +287,7 @@ igemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__
       }
       wgmma_wait<0>(acc);
       release_stage<MC>(&ctl.empty[prev], paired, rank ^ 1);
+      if (FOLD) fold_epilogue(acc, g.fold, tn * BN, g.n_out, roff);
 
       if (TMA_EPI) {
         // registers -> 128B-swizzled smem tile [128 rows][128 B] -> TMA store (coalesced, rows >= M and
@@ -989,10 +1005,11 @@ int launch_kernel(void (*kern)(P...), int grid, int threads, size_t smem, bool p
   return SIMCLR_OK;
 }
 
-template <typename T, typename To, int BN, bool A_TMA, bool SMALLC, bool TMA_EPI, bool STATS, bool MC, bool APPLY = false>
+template <typename T, typename To, int BN, bool A_TMA, bool SMALLC, bool TMA_EPI, bool STATS, bool MC, bool APPLY = false,
+          bool FOLD = false>
 int launch_igemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout, const Geom& g, double* bn_sums,
                  cudaStream_t st) {
-  auto kern = igemm_kernel<T, To, BN, A_TMA, SMALLC, TMA_EPI, STATS, MC, APPLY>;
+  auto kern = igemm_kernel<T, To, BN, A_TMA, SMALLC, TMA_EPI, STATS, MC, APPLY, FOLD>;
   { int rc = set_smem_attr(kern, Tile<BN>::SMEM_BYTES); if (rc) return rc; }   // a per-DEVICE attribute: set on every launch
   return launch_kernel(kern, igemm_grid(g, STATS), igemm_threads(A_TMA, STATS || APPLY), Tile<BN>::SMEM_BYTES, MC, st, ta, tb,
                        tout, g, bn_sums);
@@ -1004,6 +1021,26 @@ int dispatch_igemm_apply(const CUtensorMap& ta, const CUtensorMap& tb, const CUt
   typedef __nv_bfloat16 B;
   if (g.mc) return launch_igemm<B, B, BN, true, false, true, false, true, true>(ta, tb, tout, g, nullptr, st);
   return launch_igemm<B, B, BN, true, false, true, false, false, true>(ta, tb, tout, g, nullptr, st);
+}
+
+// Folded BatchNorm: bf16 activations in, bf16 (conv layers) or fp32 (the last projection-head layer, always fed by
+// TMA) out; no multicast.
+template <typename To, int BN, bool TMA_EPI>
+int dispatch_igemm_fold2(bool a_tma, bool smallc, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tout,
+                         const Geom& g, cudaStream_t st) {
+  typedef __nv_bfloat16 B;
+  if (a_tma) return launch_igemm<B, To, BN, true, false, TMA_EPI, false, false, false, true>(ta, tb, tout, g, nullptr, st);
+  if (sizeof(To) == 4) { set_error("conv2d_fprop_tc_bias: fp32 outputs need the TMA-fed kernel"); return SIMCLR_ERR_UNSUPPORTED; }
+  if (smallc) return launch_igemm<B, B, BN, false, true, TMA_EPI, false, false, false, true>(ta, tb, tout, g, nullptr, st);
+  return launch_igemm<B, B, BN, false, false, TMA_EPI, false, false, false, true>(ta, tb, tout, g, nullptr, st);
+}
+template <typename To>
+int dispatch_igemm_fold(int bn, bool a_tma, bool smallc, bool tma_epi, const CUtensorMap& ta, const CUtensorMap& tb,
+                        const CUtensorMap& tout, const Geom& g, cudaStream_t st) {
+  if (bn == 128) return tma_epi ? dispatch_igemm_fold2<To, 128, true>(a_tma, smallc, ta, tb, tout, g, st)
+                                : dispatch_igemm_fold2<To, 128, false>(a_tma, smallc, ta, tb, tout, g, st);
+  return tma_epi ? dispatch_igemm_fold2<To, 64, true>(a_tma, smallc, ta, tb, tout, g, st)
+                 : dispatch_igemm_fold2<To, 64, false>(a_tma, smallc, ta, tb, tout, g, st);
 }
 
 template <typename T, typename To, int BN, bool TMA_EPI, bool STATS>
@@ -1079,10 +1116,12 @@ inline StemGeom stem_geom(bool smallc, int mode, int64_t W, int64_t S, int64_t s
 //   gathered tensor [N][Hs][Ws][Cs]; GEMM rows = N*P*Q; weights wk [n_out][Kp]
 // `apply` (fprop with known BatchNorm coefficients: z, scale, shift, relu of a Geom): a bf16 layer fed by TMA with a
 // TMA-store epilogue writes z in the same launch and sets *applied; any other layer writes y only.
+// `fold` (fprop of folded weights, bf16 activations): `out` receives the folded epilogue's z (fold_epilogue) from
+// whichever kernel the layer lands on.
 int run_igemm(int mode, const void* src, const void* wk, void* out, int dtype, int out_dtype, int64_t N, int64_t Hs,
               int64_t Ws, int64_t Cs, int64_t P, int64_t Q, int64_t n_out, int64_t R, int64_t S, int64_t stride,
               cudaStream_t st, const char* what, double* bn_sums = nullptr, bool accum = false,
-              const Geom* apply = nullptr, int* applied = nullptr) {
+              const Geom* apply = nullptr, int* applied = nullptr, const FoldArgs* fold = nullptr) {
   const int es = dtype == SIMCLR_BF16 ? 2 : 4;
   const int KBE = 128 / es, CH = 16 / es;
   if (accum && (out_dtype != SIMCLR_F32 || bn_sums)) { set_error("%s: accumulation needs fp32 outputs and no fused statistics", what); return SIMCLR_ERR_INVALID_ARG; }
@@ -1093,11 +1132,15 @@ int run_igemm(int mode, const void* src, const void* wk, void* out, int dtype, i
   const int64_t M = N * P * Q;
   if (M >= (1ll << 31)) { set_error("%s: M too large", what); return SIMCLR_ERR_UNSUPPORTED; }
   // stem: slab of pixel pairs read through overlapping no-swizzle descriptors (tc_stem.cu)
-  if (mode == 0 && smallc && !accum && stem7x7_applicable(dtype, out_dtype, N, Hs, Ws, Cs, n_out, R, S, stride, P, Q, src, wk, out))
-    return run_stem7x7(src, wk, out, N, Hs, Ws, n_out, st, bn_sums);
+  if (fold && (mode != 0 || accum || bn_sums || dtype != SIMCLR_BF16)) {
+    set_error("%s: the folded epilogue is a bf16 fprop without statistics", what); return SIMCLR_ERR_INVALID_ARG;
+  }
+  if (mode == 0 && smallc && !accum && stem7x7_applicable(dtype, out_dtype, N, Hs, Ws, Cs, n_out, R, S, stride, P, Q, src, wk, out) &&
+      !(fold && fold->res))
+    return run_stem7x7(src, wk, out, N, Hs, Ws, n_out, st, bn_sums, fold);
   // 64 / 128-channel 3x3 stride-1 layers: halo-reuse kernel (one slab load instead of nine im2col loads)
   if (!accum && P == Hs && Q == Ws && halo3x3_applicable(dtype, out_dtype, N, Hs, Ws, Cs, n_out, R, S, stride, src, wk, out))
-    return run_halo3x3(mode, src, wk, out, N, Hs, Ws, Cs, n_out, st, bn_sums);
+    return run_halo3x3(mode, src, wk, out, N, Hs, Ws, Cs, n_out, st, bn_sums, fold);
   // Stem (4 stored channels, bf16): K runs over (r, s' in [0, S], c) with a zero slot s' = 0, i.e. the
   // filter is S+1 wide with one more pixel of left padding.  With stride 2, odd padding and an even
   // width the S+1 slots are whole 16-byte pixel pairs: the tensor is then read as [N][H][W/2][8] with
@@ -1128,7 +1171,7 @@ int run_igemm(int mode, const void* src, const void* wk, void* out, int dtype, i
   Im2colPlan pl;
   const bool a_im2col = !a_2d && !smallc && plan_im2col(mode, Hs, Ws, Cs, P, Q, R, S, stride, KBE, &pl);
   const bool a_tma = a_2d || a_im2col;
-  g.mc = a_tma ? plan_multicast(igemm_grid(g, bn_sums != nullptr), g.tiles_m, g.tiles_n, true) : 0;
+  g.mc = a_tma && !fold ? plan_multicast(igemm_grid(g, bn_sums != nullptr), g.tiles_m, g.tiles_n, true) : 0;
   const uint32_t a_box = g.mc == 1 ? 64 : 128, b_box = g.mc == 2 ? bn / 2 : bn;   // a shared tile is loaded in halves
   CUtensorMap ta, tb, tout;
   int rc = make_tmap_2d(&tb, wk, es, (uint64_t)n_out, (uint64_t)Kp, (uint64_t)Kp * es, b_box, (uint32_t)KBE);
@@ -1146,6 +1189,12 @@ int run_igemm(int mode, const void* src, const void* wk, void* out, int dtype, i
   const bool tma_epi = aligned16(out) && ((n_out * eo) % 16 == 0);
   if (tma_epi) { rc = make_tmap_2d(&tout, out, eo, (uint64_t)M, (uint64_t)n_out, (uint64_t)n_out * eo, 128, (uint32_t)(128 / eo)); if (rc) return rc; }
   else tout = tb;
+  if (fold) {
+    g.fold = *fold;
+    if (out_dtype == SIMCLR_BF16) return dispatch_igemm_fold<__nv_bfloat16>(bn, a_tma, smallc, tma_epi, ta, tb, tout, g, st);
+    if (out_dtype == SIMCLR_F32) return dispatch_igemm_fold<float>(bn, a_tma, smallc, tma_epi, ta, tb, tout, g, st);
+    set_error("%s: unsupported output dtype %d", what, out_dtype); return SIMCLR_ERR_UNSUPPORTED;
+  }
   if (apply && a_tma && tma_epi && !bn_sums && !accum && dtype == SIMCLR_BF16 && out_dtype == SIMCLR_BF16 &&
       aligned16(apply->z)) {
     g.z = apply->z; g.scale = apply->scale; g.shift = apply->shift; g.relu = apply->relu;
@@ -1410,6 +1459,22 @@ int simclr_conv2d_fprop_tc_apply(const void* x, const void* wf, void* y, void* z
   if (rc || applied) return rc;
   // the halo 3x3, stem and gathered layers: conv, then the BatchNorm apply kernel
   return simclr_bn_apply(y, dtype, nullptr, z, dtype, N * Ho * Wo, Cout, scale, shift, relu, stream);
+}
+
+int simclr_conv2d_fprop_tc_bias(const void* x, const void* wf, const float* bias, const void* residual, void* z, int z_dtype,
+                                int64_t N, int64_t H, int64_t W, int64_t Cs, int64_t Cout, int64_t R, int64_t S, int64_t stride,
+                                int relu, void* stream) {
+  SIMCLR_CHECK_ARG(x && wf && bias && z, "conv2d_fprop_tc_bias: null pointer");
+  SIMCLR_CHECK_ARG(N > 0 && H > 0 && W > 0 && Cs > 0 && Cout > 0 && R > 0 && S > 0 && (R & 1) && (S & 1) && stride > 0,
+                   "conv2d_fprop_tc_bias: bad geometry");
+  SIMCLR_CHECK_ARG(z_dtype == SIMCLR_BF16 || z_dtype == SIMCLR_F32, "conv2d_fprop_tc_bias: unknown dtype");
+  SIMCLR_CHECK_ARG(!residual || (z_dtype == SIMCLR_BF16 && Cout % 8 == 0 && aligned16(residual)),
+                   "conv2d_fprop_tc_bias: a residual needs bf16 outputs, Cout %% 8 == 0 and 16-byte alignment");
+  const int64_t Ho = (H - 1) / stride + 1, Wo = (W - 1) / stride + 1;
+  tc::FoldArgs f;
+  f.bias = bias; f.res = reinterpret_cast<const __nv_bfloat16*>(residual); f.relu = relu ? 1 : 0;
+  return tc::run_igemm(0, x, wf, z, SIMCLR_BF16, z_dtype, N, H, W, Cs, Ho, Wo, Cout, R, S, stride, (cudaStream_t)stream,
+                       "conv2d_fprop_tc_bias", nullptr, false, nullptr, nullptr, &f);
 }
 
 int simclr_conv2d_dgrad_tc(const void* dy, const void* wd, void* dx, int dtype, int dx_dtype, int64_t N, int64_t H,

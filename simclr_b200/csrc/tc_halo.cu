@@ -34,6 +34,7 @@ struct HaloGeom {
   int n_out;                   // output channels
   int tap_base, tap_sign;      // pixel offset of the A window of tap (r, s) in the slab: tap_base + tap_sign*(r*Wp + s)
   int C;                       // input channels: tap t starts at K column t*C of the packed filter
+  FoldArgs fold;               // FOLD: folded BatchNorm epilogue (fold_epilogue)
 };
 
 template <int BN, int CB, bool B_RES> struct HaloCfg {
@@ -60,7 +61,7 @@ __device__ __forceinline__ void warp_arrive_h(uint64_t* bar) {
   if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
 }
 
-template <int BN, int CB, bool B_RES, bool STATS>
+template <int BN, int CB, bool B_RES, bool STATS, bool FOLD>
 __global__ void __launch_bounds__(160, 1)
 halo3x3_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                const __grid_constant__ CUtensorMap tmap_y, const HaloGeom g, double* __restrict__ bn_sums) {
@@ -108,6 +109,24 @@ halo3x3_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant
     if (B_RES) { mbar_wait(&b_full[0], 0); }
     for (int tile = blockIdx.x; tile < g.num_tiles; tile += gridDim.x) {
       const int n = tile / g.tiles_per_img, p0 = (tile - n * g.tiles_per_img) * g.TR;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int rp = 0; rp < 2; ++rp) {
+          const int row = frag_row(h, rp), vi = row / g.Wp, vj = row - vi * g.Wp;
+          rows_in[h][rp] = vi < g.TR && vj < g.W && p0 + vi < g.H;      // outside the image: stored as zeros
+        }
+      long long roff[2][2];                                // FOLD: the thread's residual pixels
+      if (FOLD) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int rp = 0; rp < 2; ++rp) {
+            const int row = frag_row(h, rp), vi = row / g.Wp, vj = row - vi * g.Wp;
+            roff[h][rp] = rows_in[h][rp] ? (((long long)n * g.H + p0 + vi) * g.W + vj) * g.n_out : -1;
+          }
+        fold_prefetch<BN>(g.fold, 0, g.n_out, roff);
+      }
       mbar_wait(&slab_full[ss], sphase);
       const uint32_t a_tile_lo = slab0_lo + (uint32_t)ss * (CFG::SLAB_STAGE_BYTES >> 4) + (uint32_t)g.tap_base * 8u;
       int prev_bs = 0;
@@ -144,13 +163,7 @@ halo3x3_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant
       if (!B_RES) warp_arrive_h(&b_empty[prev_bs]);
       warp_arrive_h(&slab_empty[ss]);
       if (++ss == SS) { ss = 0; sphase ^= 1; }
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int rp = 0; rp < 2; ++rp) {
-          const int row = frag_row(h, rp), vi = row / g.Wp, vj = row - vi * g.Wp;
-          rows_in[h][rp] = vi < g.TR && vj < g.W && p0 + vi < g.H;      // outside the image: stored as zeros
-        }
+      if (FOLD) fold_epilogue(acc, g.fold, 0, g.n_out, roff);
 #pragma unroll
       for (int b = 0; b < BOXES; ++b, ++box_ctr) {
         uint8_t* stage = epi + (box_ctr & 1) * EPI_TILE;
@@ -391,10 +404,10 @@ int make_tmap_nhwc_tiled(CUtensorMap* map, const void* base, uint64_t N, uint64_
   return SIMCLR_OK;
 }
 
-template <int BN, int CB, bool B_RES, bool STATS>
+template <int BN, int CB, bool B_RES, bool STATS, bool FOLD = false>
 int launch_halo(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& ty, const HaloGeom& g, double* bn_sums,
                 cudaStream_t st) {
-  auto kern = halo3x3_kernel<BN, CB, B_RES, STATS>;
+  auto kern = halo3x3_kernel<BN, CB, B_RES, STATS, FOLD>;
   using CFG = HaloCfg<BN, CB, B_RES>;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CFG::SMEM);
   if (e != cudaSuccess) { set_error("halo3x3: cudaFuncSetAttribute(smem=%zu): %s", CFG::SMEM, cudaGetErrorString(e)); return (int)e; }
@@ -430,7 +443,7 @@ bool halo3x3_applicable(int dtype, int out_dtype, int64_t N, int64_t H, int64_t 
 // mode 0: fprop, wk = wf [n_out][9*C] (k = (r*3+s)*C + c).  mode 1: stride-1 dgrad, src = dY, C = Cout of the
 // conv, n_out = Cin, wk = wd [Cin][9*Cout] (k = (r*3+s)*Cout + co): dX[p,q] = sum dY[p+1-r, q+1-s] W[r,s].
 int run_halo3x3(int mode, const void* src, const void* wk, void* out, int64_t N, int64_t H, int64_t W, int64_t C,
-                int64_t n_out, cudaStream_t st, double* bn_sums) {
+                int64_t n_out, cudaStream_t st, double* bn_sums, const FoldArgs* fold) {
   HaloGeom g;
   g.H = (int)H; g.W = (int)W; g.Wp = (int)W + 2; g.TR = 128 / g.Wp; g.N = (int)N;
   g.tiles_per_img = (int)((H + g.TR - 1) / g.TR); g.num_tiles = (int)(N * g.tiles_per_img);
@@ -449,6 +462,11 @@ int run_halo3x3(int mode, const void* src, const void* wk, void* out, int64_t N,
   if (bn_sums && !accumulate_prezeroed()) {
     cudaError_t e = cudaMemsetAsync(bn_sums, 0, 2 * (size_t)n_out * sizeof(double), st);
     if (e != cudaSuccess) { set_error("halo3x3: memset: %s", cudaGetErrorString(e)); return (int)e; }
+  }
+  if (fold) {
+    g.fold = *fold;
+    return C == 64 ? launch_halo<64, 1, true, false, true>(tx, tw, ty, g, nullptr, st)
+                   : launch_halo<128, 2, false, false, true>(tx, tw, ty, g, nullptr, st);
   }
   if (!bn_sums) return C == 64 ? launch_halo<64, 1, true, false>(tx, tw, ty, g, nullptr, st)
                                 : launch_halo<128, 2, false, false>(tx, tw, ty, g, nullptr, st);

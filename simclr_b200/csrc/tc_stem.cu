@@ -32,6 +32,7 @@ struct StemGeom7 {
   int slab_stage_bytes;          // 7 * box_pairs * 16 + overread slack, 128-byte multiple
   int box_bytes;                 // bytes one TMA box delivers
   int n_out;
+  FoldArgs fold;                 // FOLD: folded BatchNorm epilogue (fold_epilogue), no residual
 };
 
 template <int BN> struct StemCfg {
@@ -52,7 +53,7 @@ __device__ __forceinline__ void warp_arrive_st(uint64_t* bar) {
   if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
 }
 
-template <int BN, bool STATS>
+template <int BN, bool STATS, bool FOLD>
 __global__ void __launch_bounds__(160, 1)
 stem7x7_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                const __grid_constant__ CUtensorMap tmap_y, const StemGeom7 g, double* __restrict__ bn_sums) {
@@ -122,6 +123,10 @@ stem7x7_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant
       wgmma_wait<0>(acc);
       warp_arrive_st(&slab_empty[ss]);
       if (++ss == SS) { ss = 0; sphase ^= 1; }
+      if (FOLD) {
+        const long long roff[2][2] = {{-1, -1}, {-1, -1}};     // no residual
+        fold_epilogue(acc, g.fold, 0, g.n_out, roff);
+      }
 #pragma unroll
       for (int b = 0; b < BOXES; ++b, ++box_ctr) {
         uint8_t* stage = epi + (box_ctr & 1) * ST_EPI_TILE;
@@ -329,10 +334,10 @@ int make_tmap_pairs(CUtensorMap* map, const void* base, uint64_t N, uint64_t H, 
   return SIMCLR_OK;
 }
 
-template <int BN, bool STATS>
+template <int BN, bool STATS, bool FOLD = false>
 int launch_stem(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& ty, const StemGeom7& g, double* bn_sums,
                 cudaStream_t st) {
-  auto kern = stem7x7_kernel<BN, STATS>;
+  auto kern = stem7x7_kernel<BN, STATS, FOLD>;
   const size_t smem = StemCfg<BN>::smem(g.slab_stage_bytes);
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) { set_error("stem7x7: cudaFuncSetAttribute(smem=%zu): %s", smem, cudaGetErrorString(e)); return (int)e; }
@@ -366,7 +371,7 @@ bool stem7x7_applicable(int dtype, int out_dtype, int64_t N, int64_t H, int64_t 
 
 // src [N][H][W][4] bf16, wk [n_out][256] (K = r*32 + slot*4 + c, slot 0 zero), out [N][P][Q][n_out] bf16
 int run_stem7x7(const void* src, const void* wk, void* out, int64_t N, int64_t H, int64_t W, int64_t n_out, cudaStream_t st,
-                double* bn_sums) {
+                double* bn_sums, const FoldArgs* fold) {
   StemGeom7 g;
   g.P = (int)(H / 2); g.Q = (int)(W / 2); g.N = (int)N; g.num_tiles = (int)(N * g.P);
   g.box_pairs = g.Q + 3; g.slab_stage_bytes = slab_stage_bytes(g.Q); g.box_bytes = 7 * g.box_pairs * 16; g.n_out = (int)n_out;
@@ -380,6 +385,10 @@ int run_stem7x7(const void* src, const void* wk, void* out, int64_t N, int64_t H
   if (bn_sums && !accumulate_prezeroed()) {
     cudaError_t e = cudaMemsetAsync(bn_sums, 0, 2 * (size_t)n_out * sizeof(double), st);
     if (e != cudaSuccess) { set_error("stem7x7: memset: %s", cudaGetErrorString(e)); return (int)e; }
+  }
+  if (fold) {
+    g.fold = *fold;
+    return n_out == 64 ? launch_stem<64, false, true>(tx, tw, ty, g, nullptr, st) : launch_stem<128, false, true>(tx, tw, ty, g, nullptr, st);
   }
   if (!bn_sums) return n_out == 64 ? launch_stem<64, false>(tx, tw, ty, g, nullptr, st) : launch_stem<128, false>(tx, tw, ty, g, nullptr, st);
   // fused statistics: one [2][n_out] partial per CTA, added into bn_sums in CTA order

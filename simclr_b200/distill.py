@@ -127,8 +127,14 @@ class Teacher:
     checkpoint, and loads every variable from `path` -- trainable ones, moving means and moving variances; a
     variable the checkpoint lacks (or holds with another shape) is an error."""
 
-    def __init__(self, path=None, num_classes=None, seed=0):
+    def __init__(self, path=None, num_classes=None, seed=0, fold_bn=None):
+        """`fold_bn` (None: --b200_fold_bn): run the teacher's conv + BatchNorm pairs folded, each one launch on
+        weights folded once, on the first forward."""
         self.flag_values = teacher_flag_values()
+        self.flag_values['b200_fold_bn'] = FLAGS.b200_fold_bn if fold_bn is None else bool(fold_bn)
+        if self.flag_values['b200_fold_bn']:
+            from .engine import get_engine
+            get_engine().check_fold_bn()
         self.path = resolve_checkpoint(path) if path is not None else None
         if num_classes is None:
             if self.path is None:

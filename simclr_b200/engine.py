@@ -188,6 +188,10 @@ class Engine:
         self._pack_ops = []
         self._pack_table = None
         self.pack_token = None
+        # conv / dense layers with a folded inference-mode BatchNorm (--b200_fold_bn), re-folded by one launch per forward
+        self._fold_ops = []
+        self._fold_table = None
+        self.fold_token = None
         # activation recomputation (resnet.BlockGroup): 'record' while a recomputed block group runs its training
         # forward (its BatchNorms keep their coefficients), 'replay' while a block re-runs that forward in the
         # backward pass (BatchNorms apply the kept coefficients: no statistics, exchange or moving-average update)
@@ -274,6 +278,39 @@ class Engine:
         if self._pack_table is None and self._pack_ops_ready() and self.conv_engine == 'tc' and \
                 not torch.cuda.is_current_stream_capturing():
             self._build_pack_table()
+
+    # -- folded BatchNorm operands (--b200_fold_bn) ---------------------------------
+    def check_fold_bn(self):
+        """Folding writes bf16 operands for the tc engine; the fp32, tc3 and simt modes have no folded path."""
+        if self.act_dtype != torch.bfloat16 or self.conv_engine != 'tc':
+            raise ValueError('--b200_fold_bn folds BatchNorm into bf16 weights for the tc engine: it needs '
+                             '--b200_precision=bf16 and --b200_conv_engine=tc (got %s, %s)'
+                             % ('bf16' if self.act_dtype == torch.bfloat16 else 'fp32', self.conv_engine))
+
+    def register_folded(self, op):
+        self._fold_ops.append(op)
+        self._fold_table = None
+
+    def fold_all(self):
+        """One launch re-folding every registered layer from its fp32 master and its BatchNorm's current moving
+        statistics (the coefficients are formed per layer first); False when the table does not exist yet (first
+        forward: layers fold themselves and `fold_done` builds the table afterwards)."""
+        if self._fold_table is None:
+            return False
+        table, n, ops = self._fold_table
+        for op in ops:
+            op.fold_bn_layer.inference_coefficients(op.fold_coef[0], op.fold_coef[1])
+        lib.fold_conv_bn_multi(table, n, stream_ptr())
+        self.fold_token = object()
+        for op in ops:
+            op.folded_token = self.fold_token
+        return True
+
+    def fold_done(self):
+        self.fold_token = None
+        if self._fold_table is None and self._fold_ops and not torch.cuda.is_current_stream_capturing():
+            rows = torch.cat([op.fold_row for op in self._fold_ops])
+            self._fold_table = (rows, len(self._fold_ops), list(self._fold_ops))
 
     @property
     def sync_bn(self):

@@ -96,6 +96,11 @@ def define_flags():
     f.DEFINE_enum('b200_jpeg_decode', 'host', ['host', 'device'],
                   'Where data.TFRecordBuilder decodes JPEGs: host (Pillow on a thread pool) or device (sm_90a '
                   'kernels, bit-exact with Pillow; other formats and unsupported JPEGs stay on the host).')
+    f.DEFINE_boolean('b200_fold_bn', False,
+                     'Inference-mode forwards (evaluation, frozen block groups and stem when fine-tuning, the '
+                     'distillation teacher) fold each BatchNorm on its moving statistics into the preceding conv or '
+                     'dense layer: one launch writes the BatchNorm (+ residual, + ReLU) output.  bf16 on the tc engine '
+                     'only.')
     f.DEFINE_integer('b200_num_classes', 1000, 'Classes of the supervised head when no dataset is read.')
     f.DEFINE_integer('b200_num_examples', 1281167, 'Examples per epoch when no dataset is read.')
     f.DEFINE_integer('b200_num_eval_examples', 50000, 'Evaluation examples when no dataset is read.')

@@ -108,6 +108,9 @@ class LinearLayer:
         assert inputs.dim() == 2, inputs.shape
         e = get_engine()
         rows = inputs.shape[0]
+        if self.use_bn and resnet.fold_bn_active(training):
+            return self.op.forward_folded(inputs.view(rows, 1, 1, self.cin), self.bn_relu, relu=relu,
+                                          out_dtype=out_dtype).view(rows, self.num_classes)
         y_dtype = out_dtype if (out_dtype is not None and not self.use_bn) else (
             torch.float32 if out_dtype == torch.float32 else None)
         sums = e.sums(2 * self.num_classes) if (self.use_bn and training) else None
@@ -260,7 +263,13 @@ class Model:
         # cast to the activation dtype and pad 3 -> 4 channels: one fused prep pass.
         features = data_util.prepare_views(inputs, num_transforms, use_blur, FLAGS.image_size,
                                            draws=self._blur_draws)
-        e.pack_all()         # bf16 operands of every conv / dense layer from the fp32 masters: one launch
+        if FLAGS.b200_fold_bn:
+            e.fold_all()     # folded operands of every inference-mode conv + BatchNorm pair: one launch
+        if not (FLAGS.b200_fold_bn and not training):
+            # bf16 operands of every conv / dense layer from the fp32 masters: one launch.  A folded inference forward
+            # reads them only in its few unfolded layers (the supervised head, an endpoint's stem conv), which then
+            # pack themselves.
+            e.pack_all()
         try:
             hiddens = self.resnet_model(features, training=training, endpoints=endpoints)
             projection_head_outputs, supervised_head_inputs = self._projection_head(hiddens, training)
@@ -273,6 +282,7 @@ class Model:
                 supervised_head_outputs = self.supervised_head(supervised_head_inputs, training)
         finally:
             e.pack_done()
+            e.fold_done()
         return projection_head_outputs, supervised_head_outputs
 
     def backward(self, d_projection_head_outputs, d_supervised_head_outputs=None):

@@ -19,6 +19,15 @@ from .engine import get_engine, BATCH_NORM_EPSILON
 from .flags_def import FLAGS
 
 
+def fold_bn_active(training):
+    """True when an inference-mode call (`training=False`: evaluation, a frozen group or stem, the teacher) runs
+    each conv -> BatchNorm pair as one launch on folded operands (--b200_fold_bn)."""
+    if training or not FLAGS.b200_fold_bn:
+        return False
+    get_engine().check_fold_bn()
+    return True
+
+
 class BatchNormRelu:  # pylint: disable=missing-docstring
     """tf2/resnet.py:31-78.  (Sync)BatchNormalization + optional ReLU; the
     residual add + ReLU of the block tail (tf2/resnet.py:382,487) can be fused in."""
@@ -52,13 +61,13 @@ class BatchNormRelu:  # pylint: disable=missing-docstring
     def _compute_statistics(self, y, training, sums):
         e = get_engine()
         C = self.C
-        rows = y.numel() // C
         st = stream_ptr()
         stats = e.empty((4, C), torch.float32)     # mean, rstd, scale, shift
         mean, rstd, scale, shift = stats[0], stats[1], stats[2], stats[3]
         g = None if self.gamma is None else self.gamma.value
         b = None if self.beta is None else self.beta.value
         if training:
+            rows = y.numel() // C
             if sums is None:
                 sums = e.sums(2 * C)
                 lib.bn_stats(y, e.code(y.dtype), rows, C, sums, st)
@@ -75,11 +84,26 @@ class BatchNormRelu:  # pylint: disable=missing-docstring
                 lib.bn_finalize(sums, count, g, b, BATCH_NORM_EPSILON, float(FLAGS.batch_norm_decay),
                                 self.moving_mean.value, self.moving_variance.value, mean, rstd, scale, shift, C, st)
         else:
-            r = torch.rsqrt(self.moving_variance.value + BATCH_NORM_EPSILON)
-            sc = r if g is None else g * r
-            mean.copy_(self.moving_mean.value); rstd.copy_(r); scale.copy_(sc)
-            shift.copy_(-self.moving_mean.value * sc if b is None else b - self.moving_mean.value * sc)
+            mean.copy_(self.moving_mean.value)
+            torch.rsqrt(self.moving_variance.value + BATCH_NORM_EPSILON, out=rstd)
+            self.inference_coefficients(scale, shift, rstd)
         return mean, rstd, scale, shift
+
+    def inference_coefficients(self, scale, shift, rstd=None):
+        """Writes the inference-mode coefficients z = y * scale + shift on the moving statistics:
+        scale = gamma * rsqrt(moving_variance + eps), shift = beta - moving_mean * scale (gamma = 1 with
+        `scale=False`, beta = 0 with `center=False`).  `rstd`: rsqrt(moving_variance + eps) if already formed."""
+        if rstd is None:
+            torch.rsqrt(self.moving_variance.value + BATCH_NORM_EPSILON, out=scale)
+        else:
+            scale.copy_(rstd)
+        if self.gamma is not None:
+            scale.mul_(self.gamma.value)
+        torch.mul(self.moving_mean.value, scale, out=shift)
+        if self.beta is None:
+            shift.neg_()
+        else:
+            torch.sub(self.beta.value, shift, out=shift)
 
     def _coefficients(self, sums, rows, mean, rstd):
         """coef [3][C] of dy = k1*dz + k2*y + k3 from the (global) backward sums; fills dgamma / dbeta."""
@@ -248,14 +272,21 @@ class ConvOp:
         self.wf = self.wd = None
         self.wf3 = self.wd3 = None           # tc3: the three bf16 terms of the packed weights
         self.packed_token = None             # == engine.pack_token: operands refreshed by the multi-layer launch
+        # --b200_fold_bn: bf16 weights with the following inference-mode BatchNorm folded in, and its bias
+        self.wfold = self.bias_f = self.fold_coef = self.fold_bn_layer = self.fold_row = None
+        self.folded_token = None             # == engine.fold_token: refreshed by the multi-layer fold launch
         self.saved_x = None
+
+    def _kp(self, es):
+        kbe = 128 // es
+        # the bf16 stem (4 stored channels) packs S+1 slots per filter row (simclr_b200.h, pack_conv_weight)
+        K = self.R * (self.S + 1 if (self.cs == 4 and es == 2) else self.S) * self.cs
+        return (K + kbe - 1) // kbe * kbe
 
     def _pack(self, e):
         es = 2 if e.act_dtype == torch.bfloat16 else 4
         kbe = 128 // es
-        # the bf16 stem (4 stored channels) packs S+1 slots per filter row (simclr_b200.h, pack_conv_weight)
-        K = self.R * (self.S + 1 if (self.cs == 4 and es == 2) else self.S) * self.cs
-        Kp = (K + kbe - 1) // kbe * kbe
+        Kp = self._kp(es)
         if self.wf is None or self.wf.dtype != e.act_dtype:
             self.wf = e.empty((self.cout, Kp))
             kd = self.R * self.S * self.cout
@@ -268,6 +299,47 @@ class ConvOp:
             return                           # refreshed by engine.pack_all() at the start of this forward
         lib.pack_conv_weight(self.kernel.value, self.wf, self.wd, e.code(e.act_dtype), self.R, self.S, self.cin,
                              self.cs, self.cout, Kp, stream_ptr())
+
+    def _fold(self, e, bn):
+        """Folded operands of this conv followed by the inference-mode BatchNorm `bn`, refreshed from the fp32
+        master and the moving statistics on every forward (a frozen teacher's: once, on its first forward)."""
+        if self.wfold is None:
+            Kp = self._kp(2)
+            self.wfold = e.empty((self.cout, Kp), torch.bfloat16)
+            self.bias_f = e.empty((self.cout,), torch.float32)
+            self.fold_coef = e.empty((2, self.cout), torch.float32)       # scale, shift
+            self.fold_bn_layer = bn
+            # the table row is written by fills with the values as kernel arguments, not copied from the host, so
+            # that a first folded forward may also run inside a CUDA-graph capture
+            self.fold_row = e.empty((1, 11), torch.int64)
+            for j, v in enumerate((self.kernel.value.data_ptr(), self.fold_coef[0].data_ptr(),
+                                   self.fold_coef[1].data_ptr(), self.wfold.data_ptr(), self.bias_f.data_ptr(),
+                                   self.R, self.S, self.cin, self.cs, self.cout, Kp)):
+                self.fold_row[0, j].fill_(v)
+            if not self.kernel.constant:
+                e.register_folded(self)
+        elif self.kernel.constant:
+            return
+        assert bn is self.fold_bn_layer
+        if e.fold_token is not None and self.folded_token is e.fold_token:
+            return                           # refreshed by engine.fold_all() at the start of this forward
+        bn.inference_coefficients(self.fold_coef[0], self.fold_coef[1])
+        lib.fold_conv_bn_multi(self.fold_row, 1, stream_ptr())
+
+    def forward_folded(self, x, bn, residual=None, relu=False, out_dtype=None):
+        """Inference forward of this conv -> BatchNorm `bn` on its moving statistics [-> + residual] [-> ReLU] as
+        ONE launch on the folded operands (simclr_conv2d_fprop_tc_bias): no conv output, no separate apply pass."""
+        e = get_engine()
+        N, H, W, Cs = x.shape
+        assert Cs == self.cs and x.dtype == torch.bfloat16, (x.shape, x.dtype, self.cs)
+        s = self.stride
+        Ho, Wo = (H - 1) // s + 1, (W - 1) // s + 1
+        self._fold(e, bn)
+        z = e.empty((N, Ho, Wo, self.cout), out_dtype or torch.bfloat16)
+        self._timed(e, 'fprop', x.shape, lambda: lib.conv2d_fprop_tc_bias(
+            x, self.wfold, self.bias_f, residual, z, e.code(z.dtype), N, H, W, Cs, self.cout, self.R, self.S, s,
+            int(relu), stream_ptr()))
+        return z
 
     def _pack3(self, e):
         """Split-bf16 operands: the three bf16 terms of every weight in the ordinary packed layouts."""
@@ -425,6 +497,10 @@ def conv_bn(conv, bn, x, training, **bn_kwargs):
     (one pass over the conv output saved per layer)."""
     e = get_engine()
     op = conv.op if hasattr(conv, 'op') else conv
+    if fold_bn_active(training):
+        relu = bn_kwargs.get('relu')
+        return op.forward_folded(x, bn, bn_kwargs.get('residual'), bn.relu if relu is None else relu,
+                                 bn_kwargs.get('out_dtype'))
     if not training:
         return bn(op.forward(x, training), training, **bn_kwargs)
     if e.recompute == 'replay' and not bn_kwargs and e.conv_engine == 'tc' and x.dtype == torch.bfloat16:
@@ -533,8 +609,12 @@ class SK_Conv2D:  # pylint: disable=invalid-name
         g32 = e.empty((N, f), torch.float32)
         lib.sk_pool(x, e.code(x.dtype), g32, N, HW, f, st)                                  # mean of the stream sum
         g = g32 if e.act_dtype == torch.float32 else self._cast(g32, e.act_dtype)
-        h = self.conv2d_0.forward(g.view(N, 1, 1, f), training).view(N, self.mid_dim)
-        h = self.batch_norm_relu_1(h, training)
+        if fold_bn_active(training):
+            h = self.conv2d_0.forward_folded(g.view(N, 1, 1, f), self.batch_norm_relu_1,
+                                             relu=self.batch_norm_relu_1.relu).view(N, self.mid_dim)
+        else:
+            h = self.conv2d_0.forward(g.view(N, 1, 1, f), training).view(N, self.mid_dim)
+            h = self.batch_norm_relu_1(h, training)
         logits = self.conv2d_1.forward(h.view(N, 1, 1, self.mid_dim), training, out_dtype=torch.float32).view(N, 2 * f)
         mixing = e.empty((N, 2 * f), torch.float32)
         out = e.empty((N, H, W, f), x.dtype)

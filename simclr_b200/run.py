@@ -36,6 +36,8 @@ class Trainer:
         from the byte model of `memory.py` (the fewest groups that make the step fit the card; none when it fits
         as it is); SIMCLR_RECOMPUTE=off / all overrides that choice."""
         self.engine = engine or engine_lib.get_engine()
+        if FLAGS.b200_fold_bn:
+            self.engine.check_fold_bn()
         self.strategy = self.engine.ctx
         self.teacher = teacher
         if teacher is not None:
